@@ -1006,7 +1006,7 @@ static void choose_config(int n_items, int S, int rows, bool bwd, int wbytes, in
 
 static int g_split_model = 1;      // tile kernels: per-decoder items only while they beat all-decoder items by wave efficiency (0: split whenever N*S <= kSplitMaxPts)
 static int g_pdl = 0;              // iteration entry points: the backward launch as a programmatic dependent of the forward launch
-static int g_fwd_f16 = 0;          // tile-kernel forward with FP16 hi|lo operands (wgmma f16, K = 16 per MMA) instead of 3xTF32; see nsb_tile.cuh mma_unit_h
+static int g_fwd_f16 = 0;          // tile-kernel forward with FP16 hi|lo operands (wgmma f16, K = 16 per MMA) instead of 3xTF32; see nsb_tile.cuh mma_rows
 static int g_wgrad_tc = 1;         // decoder weight gradients on the tensor cores when the forward kept the layer outputs (0: FP32-FMA pass)
 static int g_mlp_backend = 0;      // 0 = auto (tensor-core forward), 1 = SIMT, 2 = round-1 ray-group tensor-core kernels, 3 = tile kernels
 static size_t tc_total_smem(int max_pts, int max_rays, bool bwd = false) {

@@ -70,6 +70,8 @@ __device__ __forceinline__ uint64_t make_desc(const float* smem, uint32_t lbo_by
 // wgmma accumulates in the registers of the warpgroup that issues it, in the fragment layout of the instruction.  The kernels' epilogues
 // own one tile ROW per thread and keep several accumulators alive across MMA groups (fc_c of five layers, dL/dc and dL/d first input over all
 // layers), so every MMA group ends by storing its fragments to this CTA's accumulator slot: [column][128 rows] fp32, up to kAccCols columns.
+// (These kernels and the tile backward use it that way; the tile forward keeps its accumulators in registers and uses the slot only as
+// per-thread storage of the fc_c fragments, nsb_tile.cuh d2_frag.)
 // An accumulator address is (row << 16) | column, as the epilogues compute it: (32 * (warp & 3) << 16) + column of the thread's row.
 // Slots live in global memory (L2-resident: 2 x 132 x 128 KB); a CTA claims a free slot of its SM at start and returns it at exit.  At most
 // two tensor-core CTAs fit one SM (each takes >= 104 KB of shared memory), kAccSlotsPerSm leaves room for more.
@@ -105,6 +107,13 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit_wait() {
   asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving reads of a register accumulator above the wgmma.wait that completes it
+__device__ __forceinline__ void fence_acc(float (&d)[16]) {
+#pragma unroll
+  for (int e = 0; e < 16; e++) asm volatile("" : "+f"(d[e])::"memory");
 }
 #define NSB_WG_D16 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
                    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])

@@ -7,9 +7,11 @@
 // bumps the counters of the rays it touches after publishing its per-point results, the CTA that brings a counter to its target value
 // composites / reduces that ray from global (L2) scratch in a fixed order (bit-reproducible), and resets the counter.
 //
-// CTA = 256 threads = two threads per tile row: thread tid owns row tid & 127 and the 16-column half tid >> 7 of every 32-wide epilogue;
-// the two warpgroups execute every MMA group together (wgmma, rows [0, 64) / [64, 128)) and store the products to the CTA's accumulator slot
-// (nsb_tc.cuh, "accumulator memory"), where the epilogue threads read their rows.  Thread 0 is also the TMA producer:
+// CTA = 256 threads = two warpgroups; warpgroup g issues and waits for the MMAs of tile rows [64 g, 64 g + 64) (wgmma).  Forward: the
+// accumulators stay in registers and the epilogues work on the wgmma fragments ("register accumulators of the forward"); the point state
+// (gather, embedding) is owned row-wise: thread tid owns row tid & 127 and the 16-column half tid >> 7.  Backward: every MMA group stores
+// its products to the CTA's accumulator slot (nsb_tc.cuh, "accumulator memory"), where the row-owner epilogue reads them.  Thread 0 is also
+// the TMA producer:
 //   * weights stream through a 4-slot ring of operand UNITS (pre-split hi|lo canonical tiles, consumption order, nsb_common.cuh) with full
 //     (TMA -> MMA) and empty (MMA done -> producer) mbarriers: three units of prefetch, no thread touches a weight;
 //   * activations ping-pong between two 32 KB operand buffers; warps publish a tile by fence.proxy.async + one mbarrier.arrive per warp
@@ -168,16 +170,19 @@ __device__ __forceinline__ void issuer_wait_operands(Issuer& I, const TileSmem& 
     if (clock64() - t0 > kWaitCycles) { printf("nsb: issuer timed out waiting for operands (block %d)\n", blockIdx.x); __trap(); }
   }
 }
-// the unit the issuer is about to consume: make sure it was requested (thread 0), wait for it (all threads), return its slot base
-__device__ __forceinline__ const float* issuer_unit(Issuer& I, const TileSmem& t) {
+// unit I.issued + k (k < kSlots) of the consumption order: make sure it was requested (thread 0), wait for it (all threads), return its slot base
+__device__ __forceinline__ const float* issuer_unit(Issuer& I, const TileSmem& t, uint32_t k = 0) {
   if (threadIdx.x == 0) {
     loader_top_up(I.L, t, I.issued);
-    while (I.L.loaded <= I.issued) loader_refill(I.L, t, I.issued);
+    while (I.L.loaded <= I.issued + k) loader_refill(I.L, t, I.issued);
   }
-  const int slot = I.issued & (kSlots - 1);
-  mbar_wait_b(t.bars + B_FULL + slot, (I.issued >> 2) & 1u);
+  const uint32_t u = I.issued + k;
+  const int slot = u & (kSlots - 1);
+  mbar_wait_b(t.bars + B_FULL + slot, (u >> 2) & 1u);
   return t.ring + slot * t.slot_floats;
 }
+// slot base of unit I.issued + k (already waited for)
+__device__ __forceinline__ const float* issued_unit(const Issuer& I, const TileSmem& t, uint32_t k) { return t.ring + ((I.issued + k) & (kSlots - 1)) * t.slot_floats; }
 __device__ __forceinline__ void issuer_group_done(const TileSmem& t, int bar) {
   tc::group_done(t.bars + bar);
 }
@@ -242,19 +247,44 @@ __device__ __forceinline__ void put16_h(float* tile, int r, int cg, const float 
     *reinterpret_cast<uint4*>(hi + TM * 32 * 2) = l;
   }
 }
-// D[128 x N] (+)= A[:, ka0 .. ka0 + 16 KSTEPS) * B^T with the FP16 split.  A: [128 x 32] halves hi|lo; B: unit [N x KB] halves hi|lo.
-// (one k-step = 16 halves = two 128-byte core matrices = +16 in the start-address field, as for tf32)
-template <int KSTEPS>
-__device__ __forceinline__ void mma_unit_h(Issuer& I, const TileSmem& t, uint32_t d_tmem, const float* a, int ka0, const float* b, int N, int KB, uint32_t& acc,
-                                           uint64_t* done = nullptr) {
-  const uint32_t sbo_b = (uint32_t)(KB >> 3) * 128u;
-  const uint64_t ah = tc::make_desc(a + (ka0 >> 3) * 32, 128u, 4u * 128u);
-  const uint64_t bh = tc::make_desc(b, 128u, sbo_b);
-  const uint64_t al = ah + (uint64_t)((TM * 32 * 2) >> 4);
-  const uint64_t bl = bh + (uint64_t)((N * KB * 2) >> 4);
-  tc::wg_mma<true>(d_tmem & 0xffffu, ah, al, 4u * 128u, bh, bl, sbo_b, N, KSTEPS, acc);
-  unit_done(I, t, done);
-  acc = 1u;
+// ---- register accumulators of the forward ------------------------------------------------------------------------------------------
+// Warpgroup g issues the MMAs of its own rows [64 g, 64 g + 64) and waits for them itself, so an accumulator stays in the registers of the
+// threads that hold its wgmma m64n32 fragment (tc::frag_rc) from the first MMA to the epilogue.  A warpgroup only ever reads its own rows of
+// an A tile: tiles that the warpgroup writes from its fragments (H) need a barrier of its 128 threads only.
+// d += A[rows of this warpgroup, ka0 .. ka0 + ksteps k-steps) * B[32 c .. 32 c + 32, first ksteps k-steps]^T with the split-operand scheme (lo*hi + hi*lo + hi*hi),
+// tf32 (k-step 8) or fp16 (k-step 16, offsets in halves).  A: [128 x 32] hi|lo tile; B: unit [N x KB] hi|lo.  Issues only: the caller fences,
+// commits and waits.
+template <bool H16>
+__device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0, const float* b, int N, int KB, int c, int ksteps) {
+  const uint32_t g = (threadIdx.x >> 7) & 1u;
+  const int esz = H16 ? 2 : 4, kcm = H16 ? 8 : 4;               // bytes per element, elements per 16-byte core-matrix row
+  const uint32_t sbo_a = (32u / kcm) * 128u, sbo_b = (uint32_t)(KB / kcm) * 128u;
+  uint64_t ah = tc::make_desc(a + (ka0 / kcm) * 32, 128u, sbo_a), bh = tc::make_desc(b, 128u, sbo_b);
+  ah += (uint64_t)((8u * sbo_a * g) >> 4);
+  bh += (uint64_t)((4u * sbo_b * (uint32_t)c) >> 4);
+  const uint64_t al = ah + (uint64_t)((TM * 32 * esz) >> 4), bl = bh + (uint64_t)((N * KB * esz) >> 4);
+#pragma unroll 1
+  for (int ks = 0; ks < ksteps; ks++) {
+    const uint64_t o = 16u * (uint64_t)ks;
+    if (H16) { tc::wgmma_f16_n32(d, al + o, bh + o); tc::wgmma_f16_n32(d, ah + o, bl + o); tc::wgmma_f16_n32(d, ah + o, bh + o); }
+    else { tc::wgmma_tf32_n32(d, al + o, bh + o); tc::wgmma_tf32_n32(d, ah + o, bl + o); tc::wgmma_tf32_n32(d, ah + o, bh + o); }
+  }
+}
+// this warpgroup's MMAs on the next `count` units have completed: one arrival per warpgroup on each unit's `empty` barrier (and on `done`)
+__device__ __forceinline__ void release_units(Issuer& I, const TileSmem& t, uint32_t count, uint64_t* done = nullptr) {
+  if ((threadIdx.x & 127) == 0) {
+    for (uint32_t k = 0; k < count; k++) mbar_arrive(t.bars + B_EMPTY + ((I.issued + k) & (kSlots - 1)));
+    if (done != nullptr) mbar_arrive(done);
+  }
+  I.issued += count;
+}
+__device__ __forceinline__ void wg_bar_sync() {                 // named barrier of this warpgroup's 128 threads (ids 1, 2; 0 is __syncthreads)
+  if (threadIdx.x >> 7) asm volatile("bar.sync 2, 128;" ::: "memory");
+  else asm volatile("bar.sync 1, 128;" ::: "memory");
+}
+__device__ __forceinline__ void zero16(float (&d)[16]) {
+#pragma unroll
+  for (int e = 0; e < 16; e++) d[e] = 0.0f;
 }
 
 // ---- epilogue-side helpers -------------------------------------------------------------------------------------------------------
@@ -353,65 +383,84 @@ __device__ __forceinline__ void embed_tile(float* e_hi, const float* B, const fl
   }
 }
 
-// ---- forward: what the issuing thread (thread 0) does after the CTA published operand group I.g --------------------------------------------
-// Accumulator: D1 = [0,32), D3 = [32,64) (layer 3; its skip part is accumulated while the embedding blocks are live), D2 = [64,224) (fc_c of the five layers)
+// ---- forward: the MMA groups of one decoder, executed by every thread (each warpgroup for its own rows) ---------------------------------
+// Register accumulators: D1 (layers 0, 1, 2, 4) and D3 (layer 3: its skip part E * W3E^T is accumulated while the embedding blocks are live).
+// D2 = fc_c of the five layers is computed one 32-column chunk at a time over a whole C half and stored once, in fragment order, to this
+// thread's region of the accumulator slot (tc::s_acc): chunk i of thread tid at floats (i * kThreads + tid) * 16.  Only the thread that
+// stored a fragment reads it back (at layer i's epilogue), so the store needs no barrier.  Chunk 5 holds D3 between layer 0 and layer 3.
+__device__ __forceinline__ float4* d2_frag(int i) { return reinterpret_cast<float4*>(tc::s_acc + ((size_t)i * kThreads + threadIdx.x) * 16); }
+__device__ __forceinline__ void ld_frag(const float4* p, float (&d)[16]) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) { const float4 v = p[k]; d[4 * k] = v.x; d[4 * k + 1] = v.y; d[4 * k + 2] = v.z; d[4 * k + 3] = v.w; }
+}
+__device__ __forceinline__ void st_frag(float4* p, const float (&d)[16]) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) p[k] = make_float4(d[4 * k], d[4 * k + 1], d[4 * k + 2], d[4 * k + 3]);
+}
 template <bool H16 = false>
-__device__ __forceinline__ void issue_fc(Issuer& I, const TileSmem& t, uint32_t tmem, int half) {      // C tile `half` -> D2 += C * Wc^T (four K = 8 units)
+__device__ __forceinline__ void issue_fc(Issuer& I, const TileSmem& t, int half) {       // C tile `half` -> D2 (+)= C * Wc^T
+  constexpr int nu = H16 ? 2 : 4;                                // units of one C half: [160 x 16] FP16 / [160 x 8] tf32 (all in the ring at once)
   const int b = I.g & 1;
   issuer_wait_operands(I, t, b, (I.g >> 1) & 1u);
-  if constexpr (H16) {                                           // two [160 x 16] FP16 units
-    for (int u = 0; u < 2; u++) {
-      const float* w = issuer_unit(I, t);
-      uint32_t acc = (half == 0 && u == 0) ? 0u : 1u;
-      mma_unit_h<1>(I, t, tmem + 64u, t.a[b], 16 * u, w, 160, 16, acc, u == 1 ? t.bars + B_DONE + b : nullptr);
-    }
-  } else {
-    for (int u = 0; u < 4; u++) {
-      const float* w = issuer_unit(I, t);
-      uint32_t acc = (half == 0 && u == 0) ? 0u : 1u;
-      mma_unit<1>(I, t, tmem + 64u, t.a[b], 8 * u, w, 160, 8, 0, acc, u == 3 ? t.bars + B_DONE + b : nullptr);
-    }
+#pragma unroll 1
+  for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
+#pragma unroll 1
+  for (int c = 0; c < 5; c++) {                                  // chunk c = fc_c of layer c
+    float4* p = d2_frag(c);
+    float d[16];
+    if (half == 0) zero16(d); else ld_frag(p, d);
+    tc::wg_fence();
+#pragma unroll
+    for (int u = 0; u < nu; u++) mma_rows<H16>(d, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c, 1);
+    tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d);
+    st_frag(p, d);
   }
+  release_units(I, t, nu, t.bars + B_DONE + b);
   I.g++;
 }
 template <bool H16 = false>
-__device__ __forceinline__ void issue_l0(Issuer& I, const TileSmem& t, uint32_t tmem, int blk) {       // [D1 | D3] += E_blk * [W0_blk; W3E_blk]^T   (coarse: E = C)
+__device__ __forceinline__ void issue_l0(Issuer& I, const TileSmem& t, float (&d1)[16], float (&d3)[16]) {   // [D1 | D3] += E_blk * [W0_blk; W3E_blk]^T  (coarse: E = C)
+  constexpr int nu = H16 ? 1 : 2;                                // one [64 x 32] FP16 unit / two [64 x 16] tf32 units
   const int b = I.g & 1;
   issuer_wait_operands(I, t, b, (I.g >> 1) & 1u);
-  if constexpr (H16) {                                           // one [64 x 32] FP16 unit
-    const float* w = issuer_unit(I, t);
-    uint32_t acc = blk == 0 ? 0u : 1u;
-    mma_unit_h<2>(I, t, tmem, t.a[b], 0, w, 64, 32, acc, t.bars + B_DONE + b);
-  } else {
-    for (int h = 0; h < 2; h++) {
-      const float* w = issuer_unit(I, t);
-      uint32_t acc = (blk == 0 && h == 0) ? 0u : 1u;
-      mma_unit<2>(I, t, tmem, t.a[b], 16 * h, w, 64, 16, 0, acc, h == 1 ? t.bars + B_DONE + b : nullptr);
-    }
+#pragma unroll 1
+  for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
+  tc::wg_fence();
+#pragma unroll
+  for (int u = 0; u < nu; u++) {
+    mma_rows<H16>(d1, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 0, 2);
+    mma_rows<H16>(d3, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 1, 2);
   }
+  tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d1); tc::fence_acc(d3);
+  release_units(I, t, nu, t.bars + B_DONE + b);
   I.g++;
 }
+// layer i (1..4) of this warpgroup's rows from its rows of the H tile of layer i-1 into d1 (layer 3 accumulates onto D3); committed, not waited for
 template <bool H16 = false>
-__device__ __forceinline__ void issue_h(Issuer& I, const TileSmem& t, uint32_t tmem, int i) {          // layer i (1..4) from the H tile of layer i-1
-  const int b = I.g & 1;
-  issuer_wait_operands(I, t, b, (I.g >> 1) & 1u);
+__device__ __forceinline__ void issue_h(Issuer& I, const TileSmem& t, float (&d1)[16], const float (&d3)[16], const float* hbuf, int i) {
   const float* w = issuer_unit(I, t);
-  uint32_t acc = i == 3 ? 1u : 0u;
-  if (H16) mma_unit_h<2>(I, t, i == 3 ? tmem + 32u : tmem, t.a[b], 0, w, 32, 32, acc, t.bars + B_DONE + b);
-  else mma_unit<4>(I, t, i == 3 ? tmem + 32u : tmem, t.a[b], 0, w, 32, 32, 0, acc, t.bars + B_DONE + b);
-  I.g++;
+  if (i == 3) {
+#pragma unroll
+    for (int e = 0; e < 16; e++) d1[e] = d3[e];
+  } else {
+    zero16(d1);
+  }
+  tc::wg_fence();
+  mma_rows<H16>(d1, hbuf, 0, w, 32, 32, 0, H16 ? 2 : 4);
+  tc::wg_commit();
 }
 
-// ---- forward of one decoder: epilogue side.  n = operand-group counter (same sequence as the issuer's).  out[] = decoder outputs of this row.
+// ---- forward of one decoder.  n = operand-group counter of the groups that both warpgroups write (gather, embedding).  out[] = decoder
+// outputs of this thread's row.  masks / acts: this decoder's ReLU-mask words / layer outputs of the tile's point 0 (point stride 15 / 160), or nullptr.
 template <bool H16 = false>
-__device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t, Issuer& I, int lv, const PointGeom& G, uint32_t tmem, uint32_t& n, int hb, uint32_t hdr_parity,
-                                            float (&out)[4], uint32_t* __restrict__ gmask, float* acts = nullptr) {
+__device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t, Issuer& I, int lv, const PointGeom& G, uint32_t& n, int hb, uint32_t hdr_parity,
+                                            float (&out)[4], uint32_t* __restrict__ masks, float* __restrict__ acts, int npts) {
   const int row = threadIdx.x & (TM - 1), cg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool xyz = lv != 0;
   const int cd = op_cd(lv), no = lv == 3 ? 4 : 1;
-  const uint32_t my = ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(kCW * cg);
-  const uint32_t d1 = tmem + my, d3 = tmem + 32u + my, d2 = tmem + 64u + my;
   const float* hdr = t.hdr + hb * kHdrFloats;
+  float d1[16], d3[16];
+  zero16(d1); zero16(d3);                                        // (here, not at the first block: the compiler then sees them dead until layer 0)
   if (xyz) {
     for (int half = 0; half < cd / 32; half++) {
       if (n >= 2) wait_group(t, n - 2);
@@ -419,7 +468,7 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
       gather_tile<H16>(P.in.grid[half == 0 ? lv : 1], t.a[n & 1], G.xn, warp, lane);
       NSB_PH(1);
       publish(t, n & 1); n++;
-      issue_fc<H16>(I, t, tmem, half);
+      issue_fc<H16>(I, t, half);
       NSB_PH(2);
     }
     mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
@@ -430,73 +479,105 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
       embed_tile<H16>(t.a[n & 1], hdr + 464, G.pf, row, cg, blk);
       NSB_PH(3);
       publish(t, n & 1); n++;
-      issue_l0<H16>(I, t, tmem, blk);
+      issue_l0<H16>(I, t, d1, d3);
       NSB_PH(4);
     }
   } else {
     if (n >= 2) wait_group(t, n - 2);
     gather_tile<H16>(P.in.grid[0], t.a[n & 1], G.xnc, warp, lane);
     publish(t, n & 1); n++;
-    issue_l0<H16>(I, t, tmem, 0);
+    issue_l0<H16>(I, t, d1, d3);
     mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
   }
-  float h[kCW];
+  st_frag(d2_frag(5), d3);                                       // D3 waits for layer 3 in the slot (fewer live registers in layers 1, 2)
+  // Hidden layers.  H tiles go to buffer n & 1: its last group (n - 2) completed in both warpgroups before group n - 1 was published, and each
+  // warpgroup writes and reads only its own rows of it.
+  float* hbuf = t.a[n & 1];
+  const int wg = threadIdx.x >> 7, q = lane & 3;
+  const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);        // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8
 #pragma unroll 1
   for (int i = 0; i < 5; i++) {
-    wait_group(t, n - 1);                                        // pre-activation of layer i (and, in order, everything before it)
-    if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // the layer's weight slots are free: request the next units now, under the epilogue
+    float v2[16];
+    if (xyz) ld_frag(d2_frag(i), v2);                            // (issued before the wait: the load latency hides under layer i's MMA)
+    if (i > 0) { tc::wg_wait0(); tc::fence_acc(d1); release_units(I, t, 1); }
+    if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // the layer's weight slot is free: request the next units now, under the epilogue
     NSB_PH(7);
-    float v1[kCW];
-    acc_ld16(i == 3 ? d3 : d1, v1);
-    uint32_t m = 0;
+    // epilogue of layer i on the fragment: h = relu(D + b_i) + (D2_i + bc_i)
+    uint32_t m0 = 0, m1 = 0;                                     // ReLU bits of rows r0 / r0 + 8, this thread's columns
 #pragma unroll
-    for (int j = 0; j < kCW; j++) { const float u = v1[j] + hdr[i * 32 + kCW * cg + j]; h[j] = u > 0.0f ? u : 0.0f; m |= u > 0.0f ? (1u << j) : 0u; }
-    if (gmask != nullptr) reinterpret_cast<uint16_t*>(gmask)[i * 2 + cg] = (uint16_t)m;          // halfword cg of the 32-bit ReLU mask word
-    if (xyz) {
-      float v2[kCW];
-      acc_ld16(d2 + 32u * i, v2);
-#pragma unroll
-      for (int j = 0; j < kCW; j++) h[j] += v2[j] + hdr[160 + i * 32 + kCW * cg + j];
+    for (int e = 0; e < 16; e++) {
+      const int c = 8 * (e >> 2) + 2 * q + (e & 1);
+      const float u = d1[e] + hdr[i * 32 + c];
+      const uint32_t bit = u > 0.0f ? 1u << (8 * (e >> 2) + (e & 1)) : 0u;
+      if (e & 2) m1 |= bit; else m0 |= bit;
+      float h = u > 0.0f ? u : 0.0f;
+      if (xyz) h += v2[e] + hdr[160 + i * 32 + c];
+      d1[e] = h;
+    }
+    if (masks != nullptr) {                                      // one 32-bit word per point and layer, bit j = column j
+      m0 <<= 2 * q; m1 <<= 2 * q;
+      m0 |= __shfl_xor_sync(0xffffffffu, m0, 1); m1 |= __shfl_xor_sync(0xffffffffu, m1, 1);
+      m0 |= __shfl_xor_sync(0xffffffffu, m0, 2); m1 |= __shfl_xor_sync(0xffffffffu, m1, 2);
+      if (q == 0 && r0 < npts) masks[(size_t)r0 * 15 + i] = m0;
+      if (q == 1 && r0 + 8 < npts) masks[(size_t)(r0 + 8) * 15 + i] = m1;
     }
     if (acts != nullptr) {                                       // layer outputs kept for the tensor-core weight gradients of the backward
 #pragma unroll
-      for (int k = 0; k < kKQ; k++) __stcg(reinterpret_cast<float4*>(acts + i * 32 + 4 * k), make_float4(h[4 * k], h[4 * k + 1], h[4 * k + 2], h[4 * k + 3]));
+      for (int e = 0; e < 16; e += 2) {
+        const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q;
+        if (r < npts) __stcg(reinterpret_cast<float2*>(acts + (size_t)r * 160 + i * 32 + c), make_float2(d1[e], d1[e + 1]));
+      }
     }
     if (i == 4) break;
-    float* h_hi = t.a[n & 1];
-    if (H16) put16_h(h_hi, row, cg, h);
-    else {
+    if (i == 2) ld_frag(d2_frag(5), d3);
+    // H tile (canonical K-major, hi | lo): two adjacent columns of a row per 8-byte (tf32) / 4-byte (fp16) store
 #pragma unroll
-      for (int k = 0; k < kKQ; k++) tc::put4(h_hi, h_hi + TM * 32, row, kKQ * cg + k, 32, make_float4(h[4 * k], h[4 * k + 1], h[4 * k + 2], h[4 * k + 3]));
+    for (int e = 0; e < 16; e += 2) {
+      const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q;
+      if (H16) {
+        unsigned char* hp = reinterpret_cast<unsigned char*>(hbuf) + (((r >> 3) * 4 + (c >> 3)) * 128 + (r & 7) * 16 + (c & 7) * 2);
+        uint32_t hh, ll;
+        split_h2(d1[e], d1[e + 1], hh, ll);
+        *reinterpret_cast<uint32_t*>(hp) = hh;
+        *reinterpret_cast<uint32_t*>(hp + TM * 32 * 2) = ll;
+      } else {
+        float* hp = hbuf + tc::canon_q(r, c >> 2, 32) + (c & 3);
+        const float h0 = tc::to_tf32(d1[e]), h1 = tc::to_tf32(d1[e + 1]);
+        *reinterpret_cast<float2*>(hp) = make_float2(h0, h1);
+        *reinterpret_cast<float2*>(hp + TM * 32) = make_float2(d1[e] - h0, d1[e + 1] - h1);
+      }
     }
     NSB_PH(8);
-    publish(t, n & 1); n++;
-    issue_h<H16>(I, t, tmem, i + 1);
+    fence_proxy_async();
+    wg_bar_sync();                                               // this warpgroup's rows of H are written -> its MMA
+    issue_h<H16>(I, t, d1, d3, hbuf, i + 1);
     NSB_PH(9);
   }
   NSB_PH(8);
-  // output layer: partial dot products over this thread's columns, summed over the two threads of the row through shared memory.
-  // (buffer (n & 1) is free: its last reader was group n-2, complete.)
-  float* part = t.a[n & 1];
-  {
-    float s[4];
+  // output layer: per-row dot products over the fragment, summed over the four lanes of a row; handed to the row owners through this
+  // warpgroup's rows of the H tile (its last MMA has completed)
+  float s0[4], s1[4];
 #pragma unroll
-    for (int o = 0; o < 4; o++) {
-      s[o] = 0.0f;
-      if (o < no) {
+  for (int o = 0; o < 4; o++) {
+    s0[o] = s1[o] = 0.0f;
+    if (o < no) {
 #pragma unroll
-        for (int j = 0; j < kCW; j++) s[o] = fmaf(h[j], hdr[336 + o * 32 + kCW * cg + j], s[o]);
+      for (int e = 0; e < 16; e++) {
+        const float w = hdr[336 + o * 32 + 8 * (e >> 2) + 2 * q + (e & 1)];
+        if (e & 2) s1[o] = fmaf(d1[e], w, s1[o]); else s0[o] = fmaf(d1[e], w, s0[o]);
       }
     }
-    *reinterpret_cast<float4*>(part + (cg * TM + row) * 4) = make_float4(s[0], s[1], s[2], s[3]);
+    s0[o] += __shfl_xor_sync(0xffffffffu, s0[o], 1); s1[o] += __shfl_xor_sync(0xffffffffu, s1[o], 1);
+    s0[o] += __shfl_xor_sync(0xffffffffu, s0[o], 2); s1[o] += __shfl_xor_sync(0xffffffffu, s1[o], 2);
   }
+  constexpr int kWgHiFloats = 64 * 32 / (H16 ? 2 : 1);          // one warpgroup's rows of the hi tile
+  auto part = [&](int r) { return reinterpret_cast<float4*>(hbuf + (r >> 6) * kWgHiFloats + (r & 63) * 4); };
+  if (q == 0) *part(r0) = make_float4(s0[0], s0[1], s0[2], s0[3]);
+  if (q == 1) *part(r0 + 8) = make_float4(s1[0], s1[1], s1[2], s1[3]);
   epi_sync();
-#pragma unroll
-  for (int o = 0; o < 4; o++) out[o] = hdr[320 + o];
-#pragma unroll
-  for (int c = 0; c < kCG; c++) {
-    const float4 v = *reinterpret_cast<const float4*>(part + (c * TM + row) * 4);
-    out[0] += v.x; out[1] += v.y; out[2] += v.z; out[3] += v.w;
+  {
+    const float4 v = *part(row);
+    out[0] = hdr[320] + v.x; out[1] = hdr[321] + v.y; out[2] = hdr[322] + v.z; out[3] = hdr[323] + v.w;
   }
   epi_sync();                                                    // partials consumed before the next decoder's gather reuses the buffer
   NSB_PH(12);
@@ -945,7 +1026,9 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   NSB_PH_RESET();
   Issuer I; I.L.P = &P; I.L.q = q0; I.L.q1 = q1; I.L.k = 0; I.L.loaded = 0; I.L.mode = H16 ? 2 : 0; I.issued = 0; I.g = 0;
   if (tid == 0) {
-    for (int i = 0; i < kNumBars; i++) mbar_init(t.bars + i, (i == B_AREADY || i == B_AREADY + 1) ? kEpiThreads / 32 : 1);
+    // A_ready: one arrival per warp; empty / done: one per warpgroup (release_units)
+    for (int i = 0; i < kNumBars; i++)
+      mbar_init(t.bars + i, (i == B_AREADY || i == B_AREADY + 1) ? kEpiThreads / 32 : ((i >= B_EMPTY && i < B_EMPTY + kSlots) || i >= B_DONE) ? 2 : 1);
     mbar_fence_init();
     load_header(P, t, P.dec[q0], 0);
     for (int i = 0; i < kSlots; i++) loader_issue(I.L, t);      // (every decoder has >= 6 units)
@@ -1047,7 +1130,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
     __syncthreads();                                              // the scratch is dead: the operand buffers may be written
   }
   __syncthreads();                                                // accumulator slot + barrier initialisation visible
-  const uint32_t acc_slot = *t.tmem, tmem = 0u;        // accumulator addresses are relative to the slot (tc::s_acc)
+  const uint32_t acc_slot = *t.tmem;                              // (the slot holds the fc_c fragments, d2_frag)
   NSB_PH(44);
 
   float occ = 0.0f, c0 = 0.0f, c1 = 0.0f, c2 = 0.0f;
@@ -1056,11 +1139,11 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
     for (int qd = q0; qd < q1; qd++) {
       const int lv = P.dec[qd];
       float out[4];
-      uint32_t* gm = (P.fo.masks != nullptr && row < npts) ? P.fo.masks + ((gp0 + row) * 15 + qd * 5) : nullptr;
+      uint32_t* gm = P.fo.masks != nullptr ? P.fo.masks + (gp0 * 15 + qd * 5) : nullptr;
       const int dq = qd - q0;
       if (tid == 0 && qd + 1 < q1) load_header(P, t, P.dec[qd + 1], (dq + 1) & 1);      // (decoder qd-1 ended with CTA barriers: its buffer is free)
-      float* acts = (P.fo.acts != nullptr && lv == P.acts_lv && row < npts) ? P.fo.acts + ((gp0 + row) * 5) * 32 + kCW * cg : nullptr;
-      epi_forward<H16>(P, t, I, lv, G, tmem, n, dq & 1, (dq >> 1) & 1u, out, gm, acts);
+      float* acts = (P.fo.acts != nullptr && lv == P.acts_lv) ? P.fo.acts + gp0 * 5 * 32 : nullptr;
+      epi_forward<H16>(P, t, I, lv, G, n, dq & 1, (dq >> 1) & 1u, out, gm, acts, npts);
       if (lv == 3) { c0 = out[0]; c1 = out[1]; c2 = out[2]; } else occ += out[0];
       if (qd == 0 && cg == 0 && row < npts && P.fo.corner_idx != nullptr) {
         const nsb_grid& g = P.in.grid[lv];
@@ -1099,7 +1182,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   }
 }
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false>(P); }
-// forward with FP16 hi|lo operands (option fwd_f16; see mma_unit_h)
+// forward with FP16 hi|lo operands (option fwd_f16; see mma_rows)
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_h16_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<true>(P); }
 
 // ================================================================================================================================
