@@ -194,7 +194,7 @@ class _RenderFn(torch.autograd.Function):
         if n > 0:                                                         # (an empty batch has no storage to point at)
             _lib.check(L.nsb_render_forward(C.byref(inp), C.byref(out), _stream()), "nsb_render_forward")
         if call.aux is not None:
-            call.aux.update(z_vals=z_vals, raw=raw, corner_idx=corner)
+            call.aux.update(z_vals=z_vals, raw=raw, corner_idx=corner, masks=masks)
         ctx.call = call
         ctx.n_lvl = n_lvl
         ctx.keep = (ro, rd, depth_max, t_u, t_s, z_vals, raw, masks, split)
@@ -344,7 +344,7 @@ class FusedRenderer(object):
     # ------------------------------------------------------------------ reference API
     def render_batch_ray(self, c, decoders, rays_d, rays_o, device, stage, gt_depth=None, aux=None):
         """Render depth, uncertainty and colour of a batch of rays (Renderer.render_batch_ray, Renderer.py:63-198).
-        `aux` (optional dict) receives z_vals / raw / corner_idx for the parity tests."""
+        `aux` (optional dict) receives z_vals / raw / corner_idx / masks (the saved ReLU words) for the parity tests."""
         _require_cuda(rays_o, "rays_o")
         _require_cuda(rays_d, "rays_d")
         call, grids, plist = self._call(c, decoders, stage, gt_depth, rays_o.device, aux)
