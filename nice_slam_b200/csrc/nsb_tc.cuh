@@ -71,8 +71,8 @@ __device__ __forceinline__ uint64_t make_desc(const float* smem, uint32_t lbo_by
 // wgmma accumulates in the registers of the warpgroup that issues it, in the fragment layout of the instruction.  The kernels' epilogues
 // own one tile ROW per thread and keep several accumulators alive across MMA groups (fc_c of five layers, dL/dc and dL/d first input over all
 // layers), so every MMA group ends by storing its fragments to this CTA's accumulator slot: [column][128 rows] fp32, up to kAccCols columns.
-// (These kernels and the tile backward use it that way; the tile forward keeps its accumulators in registers and uses the slot only as
-// per-thread storage of the fc_c fragments, nsb_tile.cuh d2_frag.)
+// (These kernels use it that way; the tile kernels keep their accumulators in registers and use the slot only as per-thread storage of the
+// fragments that do not fit there -- the forward's fc_c products, the backward's first-input gradient: nsb_tile.cuh d2_frag.)
 // An accumulator address is (row << 16) | column, as the epilogues compute it: (32 * (warp & 3) << 16) + column of the thread's row.
 // Slots live in global memory (L2-resident: 2 x 132 x 128 KB); a CTA claims a free slot of its SM at start and returns it at exit.  At most
 // two tensor-core CTAs fit one SM (each takes >= 104 KB of shared memory), kAccSlotsPerSm leaves room for more.

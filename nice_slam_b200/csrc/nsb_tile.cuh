@@ -7,15 +7,15 @@
 // bumps the counters of the rays it touches after publishing its per-point results, the CTA that brings a counter to its target value
 // composites / reduces that ray from global (L2) scratch in a fixed order (bit-reproducible), and resets the counter.
 //
-// CTA = 256 threads = two warpgroups; warpgroup g issues and waits for the MMAs of tile rows [64 g, 64 g + 64) (wgmma).  Forward: the
-// accumulators stay in registers and the epilogues work on the wgmma fragments ("register accumulators of the forward"); the point state
-// (gather, embedding) is owned row-wise: thread tid owns row tid & 127 and the 16-column half tid >> 7.  Backward: every MMA group stores
-// its products to the CTA's accumulator slot (nsb_tc.cuh, "accumulator memory"), where the row-owner epilogue reads them.  Thread 0 is also
-// the TMA producer:
+// CTA = 256 threads = two warpgroups; warpgroup g issues and waits for the MMAs of tile rows [64 g, 64 g + 64) (wgmma).  In the forward
+// and the backward the accumulators stay in registers and the epilogues work on the wgmma fragments ("register accumulators of the
+// forward", "backward (input gradients)"); the point state (gather, embedding, scatter) is owned row-wise: thread tid owns row tid & 127
+// and the 16-column half tid >> 7.  Thread 0 is also the TMA producer:
 //   * weights stream through a 4-slot ring of operand UNITS (pre-split hi|lo canonical tiles, consumption order, nsb_common.cuh) with full
-//     (TMA -> MMA) and empty (MMA done -> producer) mbarriers: three units of prefetch, no thread touches a weight;
-//   * activations ping-pong between two 32 KB operand buffers; warps publish a tile by fence.proxy.async + one mbarrier.arrive per warp
-//     (A_ready), the group's MMAs run once all eight warps have arrived and signal the buffer's `done` barrier when their products are stored.
+//     (TMA -> MMA) and empty (MMA done -> producer, one arrival per warpgroup) mbarriers: three units of prefetch, no thread touches a weight;
+//   * tiles that both warpgroups write (forward: gather, embedding) ping-pong between two 32 KB operand buffers; warps publish them by
+//     fence.proxy.async + one mbarrier.arrive per warp (A_ready), and each warpgroup signals the buffer's `done` barrier when its MMAs on it
+//     have completed.  Tiles a warpgroup writes from its own fragments (H, G, DU) are published by a barrier of its 128 threads.
 // Shared memory: 64 KB activations + 40 KB ring + 6 KB headers + < 6 KB state <= 113 KB -> two CTAs per SM.
 //
 // Arithmetic is that of nsb_tc.cuh (3xTF32 split, same operand order), so results match the round-1 kernels to rounding of the output
@@ -29,7 +29,6 @@ using tc::TM;
 constexpr int kThreads = 256;                 // 8 warps = two warpgroups
 constexpr int kEpiThreads = kThreads;
 constexpr int kCG = 2, kCW = 16, kKQ = 4;      // column halves per row, columns per thread, 16-byte chunks per thread
-constexpr uint32_t kTmemCols = 256;
 constexpr int kSlots = 4;
 constexpr int kSlotFloatsFwd = 2560;          // 10 KB: the largest forward unit (fc_c: [160 x 8] hi|lo)
 constexpr int kSlotFloatsBwd = 2048;          //  8 KB: every backward unit is [32 x 32] hi|lo
@@ -66,12 +65,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void epi_sync() { __syncthreads(); }
-
-__device__ __forceinline__ void acc_ld16(uint32_t taddr, float (&v)[16]) {
-  const float* p = tc::acc_col(taddr);
-#pragma unroll
-  for (int j = 0; j < 16; j++) v[j] = p[j * TM];
-}
 
 // ---- shared memory -------------------------------------------------------------------------------------------------------------
 struct TileSmem {
@@ -183,32 +176,6 @@ __device__ __forceinline__ const float* issuer_unit(Issuer& I, const TileSmem& t
 }
 // slot base of unit I.issued + k (already waited for)
 __device__ __forceinline__ const float* issued_unit(const Issuer& I, const TileSmem& t, uint32_t k) { return t.ring + ((I.issued + k) & (kSlots - 1)) * t.slot_floats; }
-__device__ __forceinline__ void issuer_group_done(const TileSmem& t, int bar) {
-  tc::group_done(t.bars + bar);
-}
-
-// D[128 x N] (+)= A[:, ka0 .. ka0 + 8 ksteps) * B^T, 3xTF32.  A: [128 x 32] hi|lo tile; B: unit [N x KB] hi|lo, product starts at column kb0.
-// Then the unit's ring slot is released (`empty`) and, for the last unit of a group, the group's completion is signalled (`done`, or nullptr).
-__device__ __forceinline__ void unit_done(Issuer& I, const TileSmem& t, uint64_t* done) {
-  __syncthreads();                                              // every warpgroup has finished reading the slot and stored its products
-  if (threadIdx.x == 0) {
-    tc::mbar_arrive1(t.bars + B_EMPTY + (I.issued & (kSlots - 1)));
-    if (done != nullptr) tc::mbar_arrive1(done);
-  }
-  I.issued++;
-}
-template <int KSTEPS>
-__device__ __forceinline__ void mma_unit(Issuer& I, const TileSmem& t, uint32_t d_tmem, const float* a, int ka0, const float* b, int N, int KB, int kb0, uint32_t& acc,
-                                         uint64_t* done = nullptr) {
-  const uint32_t sbo_b = (uint32_t)(KB >> 2) * 128u;
-  const uint64_t ah = tc::make_desc(a + (ka0 >> 2) * 32, 128u, 8u * 128u);
-  const uint64_t bh = tc::make_desc(b + (kb0 >> 2) * 32, 128u, sbo_b);
-  const uint64_t al = ah + (uint64_t)((TM * 32 * 4) >> 4);
-  const uint64_t bl = bh + (uint64_t)((N * KB * 4) >> 4);
-  tc::wg_mma<false>(d_tmem & 0xffffu, ah, al, 8u * 128u, bh, bl, sbo_b, N, KSTEPS, acc);
-  unit_done(I, t, done);
-  acc = 1u;
-}
 
 // ---- FP16 hi|lo forward (option fwd_f16) ------------------------------------------------------------------------------------------------------
 // x = hi + lo with hi = fp16(x), lo = fp16(x - hi): 22 significant bits for |x| in [2^-3, 65504], an absolute error <= 2^-25 below (lo goes
@@ -285,6 +252,13 @@ __device__ __forceinline__ void wg_bar_sync() {                 // named barrier
 __device__ __forceinline__ void zero16(float (&d)[16]) {
 #pragma unroll
   for (int e = 0; e < 16; e++) d[e] = 0.0f;
+}
+// columns c, c + 1 (c even) of row r of a [128 x 32] tf32 operand tile (canonical K-major, hi | lo): one 8-byte store per tile
+__device__ __forceinline__ void put2(float* hi, int r, int c, float a, float b) {
+  float* hp = hi + tc::canon_q(r, c >> 2, 32) + (c & 3);
+  const float h0 = tc::to_tf32(a), h1 = tc::to_tf32(b);
+  *reinterpret_cast<float2*>(hp) = make_float2(h0, h1);
+  *reinterpret_cast<float2*>(hp + TM * 32) = make_float2(a - h0, b - h1);
 }
 
 // ---- epilogue-side helpers -------------------------------------------------------------------------------------------------------
@@ -541,10 +515,7 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
         *reinterpret_cast<uint32_t*>(hp) = hh;
         *reinterpret_cast<uint32_t*>(hp + TM * 32 * 2) = ll;
       } else {
-        float* hp = hbuf + tc::canon_q(r, c >> 2, 32) + (c & 3);
-        const float h0 = tc::to_tf32(d1[e]), h1 = tc::to_tf32(d1[e + 1]);
-        *reinterpret_cast<float2*>(hp) = make_float2(h0, h1);
-        *reinterpret_cast<float2*>(hp + TM * 32) = make_float2(d1[e] - h0, d1[e + 1] - h1);
+        put2(hbuf, r, c, d1[e], d1[e + 1]);
       }
     }
     NSB_PH(8);
@@ -608,6 +579,12 @@ __device__ __forceinline__ void put_kt16(float* hi, int lo_off, int p, int cg, c
     const int o = kt_idx(kCW * cg + j, p);
     hi[o] = h; hi[lo_off + o] = v[j] - h;
   }
+}
+// element (feature f, point p) -> hi | lo tiles
+__device__ __forceinline__ void put_kt1(float* hi, int lo_off, int f, int p, float v) {
+  const float h = tc::to_tf32(v);
+  const int o = kt_idx(f, p);
+  hi[o] = h; hi[lo_off + o] = v - h;
 }
 __device__ __forceinline__ void get_kt16(const float* hi, int lo_off, int p, int cg, float (&v)[kCW]) {      // hi + lo = the value that was split
 #pragma unroll
@@ -686,61 +663,134 @@ __device__ __forceinline__ float warp_colsum16(const float (&v)[kCW], int lane) 
   return d;
 }
 __device__ __forceinline__ int colsum_col(int lane) { return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1); }
-
-// ---- backward (input gradients): what the issuing thread does after the CTA published layer i's operands (G in a[0], DU in a[1]) ---------------
-// Accumulator: D1 = [0,32) (g of the next layer), DC = [32,96) (dL/dc), DF = [96,192) (dL/d first input).
-__device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, uint32_t tmem, int lv, int i) {
-  const bool xyz = lv != 0;
-  const int cd = op_cd(lv), nfb = op_firstp(lv) / 32;
-  issuer_wait_operands(I, t, 0, I.g & 1u);
-  if (xyz) for (int c2 = 0; c2 < cd / 32; c2++) {               // DC += G * Wc_i
-    const float* w = issuer_unit(I, t);
-    uint32_t acc = i == 4 ? 0u : 1u;
-    mma_unit<4>(I, t, tmem + 32u + 32u * c2, t.a[0], 0, w, 32, 32, 0, acc);
-  }
-  if (i >= 1) {                                                 // D1 = DU * W_i[:, hidden]
-    const float* w = issuer_unit(I, t);
-    uint32_t acc = 0u;
-    mma_unit<4>(I, t, tmem, t.a[1], 0, w, 32, 32, 0, acc);
-  }
-  if (i == 3 || i == 0) {                                       // DF += DU * W_i[:, first input]
-    for (int fb = 0; fb < nfb; fb++) {
-      const float* w = issuer_unit(I, t);
-      uint32_t acc = i == 3 ? 0u : 1u;
-      mma_unit<4>(I, t, tmem + 96u + 32u * fb, t.a[1], 0, w, 32, 32, 0, acc);
-    }
-  }
-  issuer_group_done(t, B_DONE);
-  I.g++;
+// column sums of a warp's 16 rows of an m64n32 fragment: lane l returns the sum of column frag_colsum_col(l) (the eight lanes with the same
+// l & 3 hold the same columns: reduce-scatter over lane bits 4, 3, 2)
+__device__ __forceinline__ float frag_colsum(const float (&v)[16], int lane) {
+  float a[8];                                                    // a[2 j + k] = column 8 j + 2 (l & 3) + k, both rows
+#pragma unroll
+  for (int j = 0; j < 8; j++) a[j] = v[4 * (j >> 1) + (j & 1)] + v[4 * (j >> 1) + (j & 1) + 2];
+  float b[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++) { const float give = (lane & 16) ? a[j] : a[j + 4], keep = (lane & 16) ? a[j + 4] : a[j]; b[j] = keep + __shfl_xor_sync(0xffffffffu, give, 16); }
+  float c[2];
+#pragma unroll
+  for (int j = 0; j < 2; j++) { const float give = (lane & 8) ? b[j] : b[j + 2], keep = (lane & 8) ? b[j + 2] : b[j]; c[j] = keep + __shfl_xor_sync(0xffffffffu, give, 8); }
+  const float give = (lane & 4) ? c[0] : c[1], keep = (lane & 4) ? c[1] : c[0];
+  return keep + __shfl_xor_sync(0xffffffffu, give, 4);
+}
+__device__ __forceinline__ int frag_colsum_col(int lane) {
+  const int j = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+  return 8 * (j >> 1) + 2 * (lane & 3) + (j & 1);
 }
 
-// ---- backward of one decoder: epilogue side.  Leaves dL/dc rows ([128][cd] fp32) in a[0] and the embedding-chain partials of dL/dp
-// ([2][128][4] fp32) in a[1]; the caller scatters after an epi_sync().
+// ---- backward (input gradients) ------------------------------------------------------------------------------------------------------
+// Register accumulators, as in the forward: warpgroup g issues and waits for the MMAs of its rows [64 g, 64 g + 64), and every accumulator
+// is a wgmma m64n32 fragment (tc::frag_rc) in the registers of the threads that run the epilogue on it:
+//   D1 = DU_i * W_i[:, hidden]   (dL/dh_{i-1}: from layer i's MMA to layer i-1's epilogue)
+//   DC = sum_i G_i * Wc_i        (dL/dc, accumulated over the five layers)
+//   DF = DU_3 * W_3[:, first] + DU_0 * W_0   (dL/d first input; 96 columns, the coarse decoder's 32 are dL/dc)
+// DF does not fit beside the others: its 32-column chunks live in this thread's fragment-order region of the slot (d2_frag) between layer 3
+// and layer 0, and are read back by the same thread only (no barrier).  DC keeps only the first 32 columns: the scatter reads no others (the
+// fine decoder's middle-grid features are detached), so the units of its second DC chunk are consumed without an MMA.
+struct BwdExtra {            // behind the common shared-memory part
+  double dp[TM * 3];
+  double z[TM];
+  float gocc[TM];
+  float wgt[TM];
+  float gc[kMaxTileRays * 3];
+};
+// dL/d(decoder output) of tile row r (zero beyond npts): colour decoder = compositing weight x dL/d rgb of its ray, else dL/d occupancy logit.
+// off0 = index of the tile's first point within its first ray.
+__device__ __forceinline__ void bwd_gout(const BwdExtra& X, int lv, int r, int npts, int off0, int S, float (&go)[4]) {
+  go[0] = go[1] = go[2] = go[3] = 0.0f;
+  if (r >= npts) return;
+  if (lv == 3) { const float w = X.wgt[r]; const float* gc = X.gc + 3 * ((off0 + r) / S); go[0] = w * gc[0]; go[1] = w * gc[1]; go[2] = w * gc[2]; }
+  else go[0] = X.gocc[r];
+}
+
+// Layer i of this warpgroup's rows, from its rows of the G (a[0]) and DU (a[1]) tiles: DC += G * Wc_i, D1 = DU * W_i[:, hidden] (i >= 1),
+// DF += DU * W_i[:, first input] (i = 3, 0).  A layer has up to six units (fine decoder, layer 3) for the four ring slots: they go out in waves
+// of at most kSlots units, each wave committed, waited for and released at once.  A wave carries one DF chunk (accumulator fa), two at layer 0,
+// where D1 is free to take the second: more would not fit in the registers beside D1 and DC.
+__device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, int lv, int i, float (&d1)[16], float (&dc)[16], float (&fa)[16]) {
+  const bool xyz = lv != 0;
+  const int ndc = xyz ? op_cd(lv) / 32 : 0, nd1 = i >= 1 ? 1 : 0, ndf = (i == 3 || i == 0) ? op_firstp(lv) / 32 : 0;
+  const int fmax = i == 0 ? 2 : 1;                               // DF chunks per wave
+  int f0 = 0;                                                    // first DF chunk of the wave
+  int nf = min(ndf, fmax);
+  int nu = ndc + nd1 + nf;
+#pragma unroll 1
+  for (int wave = 0; nu > 0; wave++) {
+    if (nf > 0) { if (i == 0) ld_frag(d2_frag(f0), fa); else zero16(fa); }
+    if (nf > 1) ld_frag(d2_frag(f0 + 1), d1);
+    if (wave == 0) {
+      if (xyz && i == 4) zero16(dc);
+      if (nd1) zero16(d1);
+    }
+#pragma unroll 1
+    for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
+    const int k = wave == 0 ? ndc + nd1 : 0;                     // unit of the wave's first DF chunk
+    tc::wg_fence();
+    if (wave == 0) {
+      if (xyz) mma_rows<false>(dc, t.a[0], 0, issued_unit(I, t, 0), 32, 32, 0, 4);
+      if (nd1) mma_rows<false>(d1, t.a[1], 0, issued_unit(I, t, ndc), 32, 32, 0, 4);
+    }
+    if (nf > 0) mma_rows<false>(fa, t.a[1], 0, issued_unit(I, t, k), 32, 32, 0, 4);
+    if (nf > 1) mma_rows<false>(d1, t.a[1], 0, issued_unit(I, t, k + 1), 32, 32, 0, 4);
+    tc::wg_commit(); tc::wg_wait0();
+    tc::fence_acc(dc); tc::fence_acc(d1); tc::fence_acc(fa);
+    if (nf > 0) st_frag(d2_frag(f0), fa);
+    if (nf > 1) st_frag(d2_frag(f0 + 1), d1);
+    release_units(I, t, nu);
+    f0 += nf;
+    nf = min(ndf - f0, fmax);
+    nu = nf;
+  }
+}
+
+// ---- backward of one decoder.  Leaves dL/dc rows ([128][32] fp32) in a[0] and the embedding-chain part of dL/dp ([128][4] fp32, row r at
+// a[1] + bwd_dpe_off(r)) in a[1]; the caller scatters after an epi_sync().  Each warpgroup writes both into its own rows of the operand tiles,
+// which only its own (completed) MMAs read.  masks = this decoder's ReLU-mask words of the tile's point 0 (point stride 15).
+__device__ __forceinline__ int bwd_dpe_off(int r) { return (r >> 6) * (64 * 32) + (r & 63) * 4; }
 template <bool WG>
-__device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t, Issuer& I, int lv, const PointGeom& G, uint32_t tmem, uint32_t& n, int hb, uint32_t hdr_parity,
-                                             const float (&g_out)[4], const uint32_t* __restrict__ gmask, WgSmem* w = nullptr, const float* acts_row = nullptr) {
+__device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t, Issuer& I, const BwdExtra& X, int lv, const PointGeom& G, int hb, uint32_t hdr_parity,
+                                             const uint32_t* __restrict__ masks, int npts, int off0, long long gp0, WgSmem* w = nullptr, const float* acts_row = nullptr) {
   const int row = threadIdx.x & (TM - 1), cg = threadIdx.x >> 7, warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int r0 = 64 * (threadIdx.x >> 7) + 16 * (warp & 3) + (lane >> 2);      // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8
+  const int S = P.S;
   using DW = Dec<3>;                                             // packed gradient image of the colour decoder (the only WG decoder)
   float creg[kCW];                                               // WG: this thread's 16 grid features of its point
   const bool xyz = lv != 0;
-  const int cd = op_cd(lv);
   const float* hdr = t.hdr + hb * kHdrFloats;
-  const uint16_t* gm16 = reinterpret_cast<const uint16_t*>(gmask) + cg;      // halfword cg of the five 32-bit ReLU mask words
-  const uint32_t m01 = (uint32_t)gm16[0] | ((uint32_t)gm16[2] << 16), m23 = (uint32_t)gm16[4] | ((uint32_t)gm16[6] << 16), m4 = gm16[8];
+  // ReLU bits of this thread's elements: word i of a row shifted right by 2 q puts column 8 j + 2 q + k on bit 8 j + k; row r0 + 8 goes to bits
+  // 8 j + 2 + k, and layers (0, 1) / (2, 3) share m01 / m23 (odd layer in the high nibble of each byte)
+  uint32_t m01 = 0, m23 = 0, m4 = 0;
+  {
+    const uint32_t* w0 = masks + (size_t)(r0 < npts ? r0 : npts - 1) * 15;
+    const uint32_t* w1 = masks + (size_t)(r0 + 8 < npts ? r0 + 8 : npts - 1) * 15;
+#pragma unroll
+    for (int i = 0; i < 5; i++) {
+      const uint32_t v = ((w0[i] >> (2 * q)) & 0x03030303u) | (((w1[i] >> (2 * q)) & 0x03030303u) << 2);
+      if (i == 4) m4 = v; else if (i & 2) m23 |= v << (4 * (i & 1)); else m01 |= v << (4 * (i & 1));
+    }
+  }
   mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
-  const uint32_t my = ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(kCW * cg);
-  const uint32_t dcc = tmem + 32u, dfc = tmem + 96u;
-  float* g_hi = t.a[0]; float* du_hi = t.a[1];
-  float g[kCW];
+  float d1[16], dc[16], fa[16];
+  {
+    float go0[4], go1[4];
+    bwd_gout(X, lv, r0, npts, off0, S, go0); bwd_gout(X, lv, r0 + 8, npts, off0, S, go1);
 #pragma unroll
-  for (int j = 0; j < kCW; j++) {
-    float v = 0.0f;
+    for (int e = 0; e < 16; e++) {
+      float v = 0.0f;
 #pragma unroll
-    for (int o = 0; o < 4; o++) v = fmaf(hdr[336 + o * 32 + kCW * cg + j], g_out[o], v);       // rows >= NO are zero
-    g[j] = v;
+      for (int o = 0; o < 4; o++) v = fmaf(hdr[336 + o * 32 + 8 * (e >> 2) + 2 * q + (e & 1)], (e & 2) ? go1[o] : go0[o], v);      // rows >= NO are zero
+      d1[e] = v;
+    }
   }
   if constexpr (WG) {
+    float g_out[4];
+    bwd_gout(X, lv, row, npts, off0, S, g_out);
     // grid features of this point -> registers (gathered once through the B tile)
     gather_tile_kt(P.in.grid[lv], w->b, kWgBLo, G.xn, warp, lane);
     __syncthreads();
@@ -767,30 +817,34 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
   }
 #pragma unroll 1
   for (int i = 4; i >= 0; i--) {
-    const uint32_t m = i == 4 ? m4 : (((i & 2) ? m23 : m01) >> (16 * (i & 1))) & 0xffffu;
-    if constexpr (WG) {
-      float du[kCW];
+    const uint32_t m = (i == 4 ? m4 : (i & 2) ? m23 : m01) >> (4 * (i & 1));
+    // epilogue of layer i on the fragment: g = d1, du = relu'(u_i) g -> this warpgroup's rows of the G (xyz) and DU tiles
+    float du[16];
 #pragma unroll
-      for (int j = 0; j < kCW; j++) du[j] = (m >> j) & 1u ? g[j] : 0.0f;
-      put_kt16(w->du, kWgALo, row, cg, du); put_kt16(w->g, kWgALo, row, cg, g);
-      const float sb = warp_colsum16(du, lane), sc = warp_colsum16(g, lane);      // db_i, dbc_i
-      if ((lane & 1) == 0) {
-        const int col = kCW * cg + colsum_col(lane);
-        atomicAdd(w->dpk + DW::o_b + 32 * i + col, sb); atomicAdd(w->dpk + DW::o_bc + 32 * i + col, sc);
+    for (int e = 0; e < 16; e++) du[e] = (m >> (8 * (e >> 2) + 2 * ((e >> 1) & 1) + (e & 1))) & 1u ? d1[e] : 0.0f;
+#pragma unroll
+    for (int e = 0; e < 16; e += 2) {
+      const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q;
+      if (xyz) put2(t.a[0], r, c, d1[e], d1[e + 1]);
+      put2(t.a[1], r, c, du[e], du[e + 1]);
+    }
+    if constexpr (WG) {                                          // the same values transposed ([feature][point]) and their column sums: db_i, dbc_i
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q + (e & 1);
+        put_kt1(w->du, kWgALo, c, r, du[e]); put_kt1(w->g, kWgALo, c, r, d1[e]);
       }
+      const float sb = frag_colsum(du, lane), sc = frag_colsum(d1, lane);
+      const int col = frag_colsum_col(lane);
+      atomicAdd(w->dpk + DW::o_b + 32 * i + col, sb); atomicAdd(w->dpk + DW::o_bc + 32 * i + col, sc);
     }
-#pragma unroll
-    for (int k = 0; k < kKQ; k++) {
-      if (xyz) tc::put4(g_hi, g_hi + TM * 32, row, kKQ * cg + k, 32, make_float4(g[4 * k], g[4 * k + 1], g[4 * k + 2], g[4 * k + 3]));
-      tc::put4(du_hi, du_hi + TM * 32, row, kKQ * cg + k, 32,
-               make_float4((m >> (4 * k)) & 1u ? g[4 * k] : 0.0f, (m >> (4 * k + 1)) & 1u ? g[4 * k + 1] : 0.0f,
-                           (m >> (4 * k + 2)) & 1u ? g[4 * k + 2] : 0.0f, (m >> (4 * k + 3)) & 1u ? g[4 * k + 3] : 0.0f));
-    }
+    fence_proxy_async();
+    wg_bar_sync();                                               // this warpgroup's rows of G / DU are written -> its MMAs
     NSB_PH(22);
-    publish(t, 0);
-    issue_bwd_layer(I, t, tmem, lv, i);
+    issue_bwd_layer(I, t, lv, i, d1, dc, fa);
+    if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // slots of this layer are free: fetch the next layer's units under the epilogue
     NSB_PH(23);
-    if constexpr (WG) {                                          // weight gradients of layer i (the chain's MMAs run meanwhile)
+    if constexpr (WG) {                                          // weight gradients of layer i
       if (i >= 1) {                                              // hidden input H_{i-1}
         float xr[kCW];
 #pragma unroll
@@ -818,26 +872,17 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
           wg_group(*w, 0, w->dpk + (i == 0 ? DW::o_W0 : DW::o_W3E) + 32 * blk, DW::PF, 32);
         }
       }
+      NSB_PH(24);
     }
-    mbar_wait_b(t.bars + B_DONE, n & 1u); n++;
-    if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // slots of this layer are free: fetch the next layer's units under the epilogue
-    NSB_PH(24);
-    if (i >= 1) acc_ld16(tmem + my, g);
   }
-  NSB_PH(22);
-  // dL/dc rows -> a[0] (plain fp32 [128][cd]); every MMA reading the buffers has completed
-  float* dcs = t.a[0];
-  {
-    float v[kCW];
-    const int nch = xyz ? (cd >> 5) : 1;
-    for (int c = 0; c < nch; c++) {
-      acc_ld16((xyz ? dcc : dfc) + 32u * c + my, v);
+  // dL/dc rows -> a[0] (plain fp32 [128][32]): DC, or the coarse decoder's DF
+  if (!xyz) ld_frag(d2_frag(0), dc);
 #pragma unroll
-      for (int k = 0; k < kKQ; k++)
-        *reinterpret_cast<float4*>(dcs + row * cd + 32 * c + kCW * cg + 4 * k) = make_float4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-    }
+  for (int e = 0; e < 16; e += 2) {
+    const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q;
+    *reinterpret_cast<float2*>(t.a[0] + r * 32 + c) = make_float2(dc[e], dc[e + 1]);
   }
-  float dpe[3] = {0.0f, 0.0f, 0.0f};
+  float dpe0[3] = {0.0f, 0.0f, 0.0f}, dpe1[3] = {0.0f, 0.0f, 0.0f};          // rows r0, r0 + 8
   if (xyz) {
     const float* B = hdr + 464;
     if constexpr (WG) {                                          // B tile of the dB groups: the point's coordinates in columns 0..2
@@ -846,37 +891,58 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       for (int j = 0; j < kCW; j++) pv[j] = (cg == 0 && j < 3) ? G.pf[j] : 0.0f;
       put_kt16(w->b, kWgBLo, row, cg, pv);
     }
-    for (int c = 0; c < 3; c++) {
-      float v[kCW];
-      acc_ld16(dfc + 32u * c + my, v);
-      float dxv[kCW];
+    float pf0[3], pf1[3];                                        // embedding inputs of the fragment's rows (make_point, as the row owners did)
+    {
+      float o[3], d[3];
+      PointGeom Gr;
+      const int l0 = r0 < npts ? r0 : npts - 1, l1 = r0 + 8 < npts ? r0 + 8 : npts - 1;
+      const int ray0 = (int)((gp0 + l0) / S), ray1 = (int)((gp0 + l1) / S);
 #pragma unroll
-      for (int j = 0; j < kCW; j++) {
-        const int f = 32 * c + kCW * cg + j;
-        dxv[j] = 0.0f;
+      for (int a = 0; a < 3; a++) { o[a] = P.in.rays_o[3 * ray0 + a]; d[a] = P.in.rays_d[3 * ray0 + a]; }
+      make_point(P.in.bound, P.in.coarse_bound, o, d, X.z[r0], Gr);
+      pf0[0] = Gr.pf[0]; pf0[1] = Gr.pf[1]; pf0[2] = Gr.pf[2];
+#pragma unroll
+      for (int a = 0; a < 3; a++) { o[a] = P.in.rays_o[3 * ray1 + a]; d[a] = P.in.rays_d[3 * ray1 + a]; }
+      make_point(P.in.bound, P.in.coarse_bound, o, d, X.z[r0 + 8], Gr);
+      pf1[0] = Gr.pf[0]; pf1[1] = Gr.pf[1]; pf1[2] = Gr.pf[2];
+    }
+    for (int c = 0; c < 3; c++) {
+      ld_frag(d2_frag(c), fa);
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        const int f = 32 * c + 8 * (e >> 2) + 2 * q + (e & 1);
+        float dx = 0.0f;
         if (f < kEmb) {
+          const float* pf = (e & 2) ? pf1 : pf0;
+          float* dpe = (e & 2) ? dpe1 : dpe0;
           const float b0 = B[f], b1 = B[kEmbPad + f], b2 = B[2 * kEmbPad + f];
-          float x = G.pf[0] * b0; x = fmaf(G.pf[1], b1, x); x = fmaf(G.pf[2], b2, x);
-          const float dx = __cosf(reduce_2pi(x)) * v[j];
-          dxv[j] = dx;
+          float x = pf[0] * b0; x = fmaf(pf[1], b1, x); x = fmaf(pf[2], b2, x);
+          dx = __cosf(reduce_2pi(x)) * fa[e];
           dpe[0] = fmaf(b0, dx, dpe[0]); dpe[1] = fmaf(b1, dx, dpe[1]); dpe[2] = fmaf(b2, dx, dpe[2]);
         }
+        if constexpr (WG) put_kt1(w->du, kWgALo, f - 32 * c, r0 + 8 * ((e >> 1) & 1), dx);
       }
       if constexpr (WG) {                                        // dB[a][f] = sum_p p_a cos(.) dE_f  (embedder._B is a parameter of the decoder)
-        put_kt16(w->du, kWgALo, row, cg, dxv);
         const int nf = kEmb - 32 * c < 32 ? kEmb - 32 * c : 32;
         wg_group(*w, 0, w->dpk + DW::o_B + 32 * c, kEmbPad, nf, true);
       }
     }
   }
-  *reinterpret_cast<float4*>(t.a[1] + (cg * TM + row) * 4) = make_float4(dpe[0], dpe[1], dpe[2], 0.0f);
+  // per-row sums over the four lanes of a row
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    dpe0[a] += __shfl_xor_sync(0xffffffffu, dpe0[a], 1); dpe1[a] += __shfl_xor_sync(0xffffffffu, dpe1[a], 1);
+    dpe0[a] += __shfl_xor_sync(0xffffffffu, dpe0[a], 2); dpe1[a] += __shfl_xor_sync(0xffffffffu, dpe1[a], 2);
+  }
+  if (q == 0) *reinterpret_cast<float4*>(t.a[1] + bwd_dpe_off(r0)) = make_float4(dpe0[0], dpe0[1], dpe0[2], 0.0f);
+  if (q == 1) *reinterpret_cast<float4*>(t.a[1] + bwd_dpe_off(r0 + 8)) = make_float4(dpe1[0], dpe1[1], dpe1[2], 0.0f);
   NSB_PH(27);
 }
 
-// Backward of gather_tile (same warp -> rows mapping).  dcs = [128][cd] fp32.  emit(row, gx) once per point.
+// Backward of gather_tile (same warp -> rows mapping).  dcs = [128][32] fp32.  emit(row, gx) once per point.
 template <typename F>
 __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restrict__ dgrid, const int32_t* __restrict__ slots,
-                                             const float* dcs, int cd, const float xn[3], int warp, int lane, F&& emit) {
+                                             const float* dcs, const float xn[3], int warp, int lane, F&& emit) {
   const bool fast = grid_fast(g);
   const int q = lane & 7, qd = warp & 3, it0 = (warp >> 2) * 4;
 #pragma unroll 1
@@ -886,7 +952,7 @@ __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restric
     float x[3];
     x[0] = __shfl_sync(0xffffffffu, xn[0], src_lane); x[1] = __shfl_sync(0xffffffffu, xn[1], src_lane); x[2] = __shfl_sync(0xffffffffu, xn[2], src_lane);
     const Tri t = make_tri(x, g.W, g.H, g.D);
-    const float4 d4 = *reinterpret_cast<const float4*>(dcs + row * cd + 4 * q);
+    const float4 d4 = *reinterpret_cast<const float4*>(dcs + row * 32 + 4 * q);
     const float dc[4] = {d4.x, d4.y, d4.z, d4.w};
     float gi[3] = {0.f, 0.f, 0.f};
     float4 vv[8];
@@ -1188,16 +1254,6 @@ __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_h16_kernel(co
 // ================================================================================================================================
 // backward kernel (input gradients: rays + grid voxels)
 // ================================================================================================================================
-namespace tl {
-struct BwdExtra {            // behind the common shared-memory part
-  double dp[TM * 3];
-  double z[TM];
-  float gocc[TM];
-  float wgt[TM];
-  float gc[kMaxTileRays * 3];
-};
-}  // namespace tl
-
 // WG = true: the item's decoder (the colour decoder) also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the
 // "tensor-core weight gradients" helpers): 96 KB more shared memory in front of the common part -> one CTA per SM.
 template <bool WG>
@@ -1228,7 +1284,8 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   NSB_PH_RESET();
   Issuer I; I.L.P = &P; I.L.q = q0; I.L.q1 = q1; I.L.k = 0; I.L.loaded = 0; I.L.mode = 1; I.issued = 0; I.g = 0;
   if (tid == 0) {
-    for (int i = 0; i < kNumBars; i++) mbar_init(t.bars + i, (i == B_AREADY || i == B_AREADY + 1) ? kEpiThreads / 32 : 1);
+    // empty: one arrival per warpgroup (release_units); A_ready / done are not used by the backward
+    for (int i = 0; i < kNumBars; i++) mbar_init(t.bars + i, (i >= B_EMPTY && i < B_EMPTY + kSlots) ? 2 : 1);
     mbar_fence_init();
     load_header(P, t, P.dec[q0], 0);
     for (int i = 0; i < kSlots; i++) loader_issue(I.L, t);
@@ -1306,32 +1363,26 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
     if (cg == 0) X.z[row] = z;
   }
   __syncthreads();                                                // prologue scratch dead, gocc / wgt / gc visible, accumulator slot + barriers visible
-  const uint32_t acc_slot = *t.tmem, tmem = 0u;        // accumulator addresses are relative to the slot (tc::s_acc)
+  const uint32_t acc_slot = *t.tmem;                              // (the slot holds the DF fragments between layers 3 and 0, d2_frag)
   NSB_PH(21);
 
   {
-    uint32_t n = 0;
+    const int off0 = (int)(gp0 - (long long)ray_lo * S);
     for (int qd = q0; qd < q1; qd++) {
       const int lv = P.dec[qd];
-      const uint32_t* gm = P.bw.masks + ((gp0 + lp) * 15 + P.dec_pos[qd] * 5);
-      float g_out[4] = {0.f, 0.f, 0.f, 0.f};
-      if (row < npts) {
-        if (lv == 3) { const float w = X.wgt[row]; const float* gc = X.gc + 3 * (rayr - ray_lo); g_out[0] = w * gc[0]; g_out[1] = w * gc[1]; g_out[2] = w * gc[2]; }
-        else g_out[0] = X.gocc[row];
-      }
+      const uint32_t* gm = P.bw.masks + (gp0 * 15 + P.dec_pos[qd] * 5);
       const int dq = qd - q0;
       if (tid == 0 && qd + 1 < q1) load_header(P, t, P.dec[qd + 1], (dq + 1) & 1);      // (the previous decoder ended with CTA barriers: its buffer is free)
       const float* acts_row = (WG && row < npts) ? P.bw.acts + ((gp0 + row) * 5) * 32 + kCW * cg : nullptr;
-      epi_backward<WG>(P, t, I, lv, G, tmem, n, dq & 1, (dq >> 1) & 1u, g_out, gm, WG ? &wg : nullptr, acts_row);
+      epi_backward<WG>(P, t, I, X, lv, G, dq & 1, (dq >> 1) & 1u, gm, npts, off0, gp0, WG ? &wg : nullptr, acts_row);
       epi_sync();                                                 // dL/dc rows + embedding partials visible
       const double* bb = lv == 0 ? P.in.coarse_bound : P.in.bound;
       const double sc[3] = {2.0 / (bb[1] - bb[0]), 2.0 / (bb[3] - bb[2]), 2.0 / (bb[5] - bb[4])};      // d(normalised)/dp, common.py:280-282
       const float* xn = lv == 0 ? G.xnc : G.xn;
-      scatter_tile(P.in.grid[lv], P.bw.d_grid[lv], P.bw.slot_map[lv], t.a[0], op_cd(lv), xn, warp, lane, [&](int prow, const float gx[3]) {
+      scatter_tile(P.in.grid[lv], P.bw.d_grid[lv], P.bw.slot_map[lv], t.a[0], xn, warp, lane, [&](int prow, const float gx[3]) {
         if (prow < npts) {
-          const float4 p0 = *reinterpret_cast<const float4*>(t.a[1] + prow * 4);
-          const float4 p1 = *reinterpret_cast<const float4*>(t.a[1] + (TM + prow) * 4);
-          const float dpe[3] = {p0.x + p1.x, p0.y + p1.y, p0.z + p1.z};
+          const float4 p = *reinterpret_cast<const float4*>(t.a[1] + bwd_dpe_off(prow));
+          const float dpe[3] = {p.x, p.y, p.z};
 #pragma unroll
           for (int a = 0; a < 3; a++) X.dp[3 * prow + a] += (double)dpe[a] + (double)gx[a] * sc[a];
         }

@@ -18,7 +18,7 @@ TILE_NAMES = {40: "fwd: launch -> depth max done", 41: "fwd: ray table (bbox far
               1: "fwd: gather (per grid)", 2: "fwd: publish + issue fc_c", 6: "fwd: wait free buffer (E block)", 3: "fwd: embed block compute", 4: "fwd: publish + issue layer-0 block",
               7: "fwd: wait MMAs of the layer", 8: "fwd: layer epilogue (relu, masks, H write)", 9: "fwd: publish + issue hidden layer", 12: "fwd: output layer + syncs",
               14: "fwd: dealloc + sync", 15: "fwd: parts store + ray completion", 16: "fwd: compositing of completed rays",
-              20: "bwd: launch -> ray prologue (weights, dL/docc)", 21: "bwd: point geometry + sync", 22: "bwd: G/DU operand write", 23: "bwd: publish + issue layer", 24: "bwd: wait MMAs",
+              20: "bwd: launch -> ray prologue (weights, dL/docc)", 21: "bwd: point geometry + sync", 22: "bwd: layer epilogue (G/DU write)", 23: "bwd: issue + wait layer MMAs", 24: "bwd: weight-gradient groups (WG)",
               27: "bwd: dc rows + cos chain", 29: "bwd: scatter + dp", 30: "bwd: per-ray partial sums", 31: "bwd: ray completion", 32: "bwd: final ray reduce"}
 NAMES = {0: "fwd: tail sync of previous decoder", 1: "fwd: gather", 2: "fwd: fc_c publish + issue", 3: "fwd: E block 0", 4: "fwd: E block 1",
          5: "fwd: E block 2", 6: "fwd: wait fc_c / layer-0 MMAs", 7: "fwd: layer step 0", 8: "fwd: layer step 1", 9: "fwd: layer step 2",
