@@ -239,7 +239,7 @@ __global__ void batch_max_kernel(const float* __restrict__ gt, int n, float* __r
     if ((int)threadIdx.x < px.world) ll_put_f32(px.peer[threadIdx.x] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + px.rank) * 16, out2[0], seq);
     if (threadIdx.x < 32) {
       float mm = -INFINITY;
-      if ((int)threadIdx.x < px.world) mm = ll_get_f32(px.peer[px.rank] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + threadIdx.x) * 16, seq, px, 0);
+      if ((int)threadIdx.x < px.world) mm = ll_get_f32(px.peer[px.rank] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + threadIdx.x) * 16, seq);
       for (int o = 16; o > 0; o >>= 1) mm = fmaxf(mm, __shfl_xor_sync(0xffffffffu, mm, o));
       if (threadIdx.x == 0) { out2[0] = mm; out2[1] = __fmul_rn(mm, 1.2f); }
     }

@@ -33,14 +33,15 @@ __device__ __forceinline__ void ll_put(unsigned char* slot16, double v, uint32_t
   const unsigned long long w0 = ((unsigned long long)seq << 32) | (b & 0xffffffffull), w1 = ((unsigned long long)seq << 32) | (b >> 32);
   asm volatile("st.relaxed.sys.global.v2.u64 [%0], {%1, %2};" ::"l"(slot16), "l"(w0), "l"(w1) : "memory");
 }
-__device__ __forceinline__ double ll_get(const unsigned char* slot16, uint32_t seq, const PeerX& px, int c) {
+__device__ __forceinline__ double ll_get(const unsigned char* slot16, uint32_t seq) {
   unsigned long long w0, w1;
   const long long t0 = clock64();
   for (;;) {
     asm volatile("ld.relaxed.sys.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(slot16) : "memory");
     if ((uint32_t)(w0 >> 32) == seq && (uint32_t)(w1 >> 32) == seq) break;
-    // a rank that never arrives (crashed process, mismatched call sequence) must not hang the device: fail the launch instead
-    if (clock64() - t0 > kPeerWaitCycles) { printf("nsb: peer exchange timed out (rank %d, channel %d, seq %u)\n", px.rank, c, seq); __trap(); }
+    // a rank that never arrives (crashed process, mismatched call sequence) must not hang the device: fail the launch instead (no printf:
+    // these waits run inside wgmma kernels, see nsb_tile.cuh mbar_wait_b)
+    if (clock64() - t0 > kPeerWaitCycles) __trap();
   }
   return __longlong_as_double((long long)((w1 << 32) | (w0 & 0xffffffffull)));
 }
@@ -49,13 +50,13 @@ __device__ __forceinline__ void ll_put_f32(unsigned char* slot8, float v, uint32
   const unsigned long long w = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint(v);
   asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(slot8), "l"(w) : "memory");
 }
-__device__ __forceinline__ float ll_get_f32(const unsigned char* slot8, uint32_t seq, const PeerX& px, int c) {
+__device__ __forceinline__ float ll_get_f32(const unsigned char* slot8, uint32_t seq) {
   unsigned long long w;
   const long long t0 = clock64();
   for (;;) {
     asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(w) : "l"(slot8) : "memory");
     if ((uint32_t)(w >> 32) == seq) break;
-    if (clock64() - t0 > kPeerWaitCycles) { printf("nsb: peer exchange timed out (rank %d, channel %d, seq %u)\n", px.rank, c, seq); __trap(); }
+    if (clock64() - t0 > kPeerWaitCycles) __trap();
   }
   return __uint_as_float((uint32_t)w);
 }
@@ -85,7 +86,7 @@ __device__ __forceinline__ float peer_max_all_ctas(const PeerX& px, float local,
     ll_put_f32(px.peer[threadIdx.x] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + px.rank) * 16, local, seq);
   float m = -INFINITY;
   if (threadIdx.x < 32) {                                    // warp 0: lane r polls rank r's word, then the maximum over the lanes
-    if ((int)threadIdx.x < px.world) m = ll_get_f32(px.peer[px.rank] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + threadIdx.x) * 16, seq, px, 0);
+    if ((int)threadIdx.x < px.world) m = ll_get_f32(px.peer[px.rank] + kXMaxOff + ((size_t)par * NSB_MAX_PEERS + threadIdx.x) * 16, seq);
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (threadIdx.x == 0) *reinterpret_cast<float*>(s_seq) = m;
   }
@@ -107,7 +108,7 @@ __device__ __forceinline__ void peer_sum13(const PeerX& px, const double* tot, i
   }
   if ((int)threadIdx.x < n_val) {
     double v = 0.0;
-    for (int r = 0; r < px.world; r++) v += ll_get(px.peer[px.rank] + kXSumOff + ((size_t)par * NSB_MAX_PEERS + r) * kXSumStride + (size_t)threadIdx.x * 16, seq, px, 2);
+    for (int r = 0; r < px.world; r++) v += ll_get(px.peer[px.rank] + kXSumOff + ((size_t)par * NSB_MAX_PEERS + r) * kXSumStride + (size_t)threadIdx.x * 16, seq);
     out[threadIdx.x] = v;
   }
   peer_end(px, 2, seq);
@@ -167,7 +168,7 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
       double* plain = reinterpret_cast<double*>(px.peer[px.rank] + peer_pool_plain_off(px.max_n));
       for (int i = threadIdx.x; i < n * px.world; i += blockDim.x) {
         const int r = i / n, j = i - r * n;
-        plain[(size_t)r * px.max_n + j] = ll_get(px.peer[px.rank] + kXPoolOff + (((size_t)par * NSB_MAX_PEERS + r) * px.max_n + j) * 16, seq, px, 1);
+        plain[(size_t)r * px.max_n + j] = ll_get(px.peer[px.rank] + kXPoolOff + (((size_t)par * NSB_MAX_PEERS + r) * px.max_n + j) * 16, seq);
       }
       peer_end(px, 1, seq);                                  // (its barrier also makes `plain` visible to the whole CTA)
       mp = plain;

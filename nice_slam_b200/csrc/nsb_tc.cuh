@@ -86,7 +86,7 @@ __shared__ float* s_acc;                       // this CTA's slot
 __device__ __forceinline__ uint32_t acc_acquire() {
   uint32_t smid;
   asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-  if (smid >= (uint32_t)kAccMaxSm) { printf("nsb: SM id %u beyond the accumulator pool\n", smid); __trap(); }
+  if (smid >= (uint32_t)kAccMaxSm) __trap();                    // SM id beyond the pool (no printf in wgmma kernels: nsb_tile.cuh mbar_wait_b)
   const long long t0 = clock64();
   for (;;) {
     for (int k = 0; k < kAccSlotsPerSm; k++) {
@@ -97,7 +97,7 @@ __device__ __forceinline__ uint32_t acc_acquire() {
         return (uint32_t)s;
       }
     }
-    if (clock64() - t0 > 4000000000ll) { printf("nsb: no free accumulator slot on SM %u\n", smid); __trap(); }
+    if (clock64() - t0 > 4000000000ll) __trap();                // no free accumulator slot on this SM
   }
 }
 // thread 0, after a CTA barrier that follows the last accumulator access

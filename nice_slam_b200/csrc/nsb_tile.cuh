@@ -53,12 +53,13 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
                : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-// bounded wait: a protocol error traps (the launch fails with an error) instead of hanging the device
+// bounded wait: a protocol error traps (the launch fails with an error) instead of hanging the device.  No printf here or anywhere else in
+// a wgmma kernel: a call to it makes ptxas serialize every wgmma of the kernel (C7510).
 __device__ __forceinline__ void mbar_wait_b(uint64_t* bar, uint32_t parity) {
   if (mbar_try(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try(bar, parity)) {
-    if (clock64() - t0 > kWaitCycles) { printf("nsb: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x, (void*)bar, parity); __trap(); }
+    if (clock64() - t0 > kWaitCycles) __trap();
   }
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -160,7 +161,7 @@ __device__ __forceinline__ void issuer_wait_operands(Issuer& I, const TileSmem& 
   const long long t0 = clock64();
   while (!mbar_test(bar, parity)) {                              // poll: the ring is topped up between polls
     if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);
-    if (clock64() - t0 > kWaitCycles) { printf("nsb: issuer timed out waiting for operands (block %d)\n", blockIdx.x); __trap(); }
+    if (clock64() - t0 > kWaitCycles) __trap();
   }
 }
 // unit I.issued + k (k < kSlots) of the consumption order: make sure it was requested (thread 0), wait for it (all threads), return its slot base
@@ -221,8 +222,13 @@ __device__ __forceinline__ void put16_h(float* tile, int r, int cg, const float 
 // d += A[rows of this warpgroup, ka0 .. ka0 + ksteps k-steps) * B[32 c .. 32 c + 32, first ksteps k-steps]^T with the split-operand scheme (lo*hi + hi*lo + hi*hi),
 // tf32 (k-step 8) or fp16 (k-step 16, offsets in halves).  A: [128 x 32] hi|lo tile; B: unit [N x KB] hi|lo.  Issues only: the caller fences,
 // commits and waits.
-template <bool H16>
-__device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0, const float* b, int N, int KB, int c, int ksteps) {
+// MMA groups are kept in a form ptxas can pipeline (otherwise it waits for every wgmma before issuing the next, C7517-C7520): between
+// wgmma.fence and commit_group a straight run of wgmma with compile-time unit and k-step counts, reached by every thread of the warpgroup;
+// accumulators initialised just before the fence (a constant zero kept in the open, as in the coarse layer 0, is materialised by ptxas
+// inside the group, hence zero16_opaque); producer work and mbarrier waits before them; every group waited for on every path that leads
+// to a read of its accumulators.
+template <bool H16, int ksteps>
+__device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0, const float* b, int N, int KB, int c) {
   const uint32_t g = (threadIdx.x >> 7) & 1u;
   const int esz = H16 ? 2 : 4, kcm = H16 ? 8 : 4;               // bytes per element, elements per 16-byte core-matrix row
   const uint32_t sbo_a = (32u / kcm) * 128u, sbo_b = (uint32_t)(KB / kcm) * 128u;
@@ -230,7 +236,7 @@ __device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0
   ah += (uint64_t)((8u * sbo_a * g) >> 4);
   bh += (uint64_t)((4u * sbo_b * (uint32_t)c) >> 4);
   const uint64_t al = ah + (uint64_t)((TM * 32 * esz) >> 4), bl = bh + (uint64_t)((N * KB * esz) >> 4);
-#pragma unroll 1
+#pragma unroll
   for (int ks = 0; ks < ksteps; ks++) {
     const uint64_t o = 16u * (uint64_t)ks;
     if (H16) { tc::wgmma_f16_n32(d, al + o, bh + o); tc::wgmma_f16_n32(d, ah + o, bl + o); tc::wgmma_f16_n32(d, ah + o, bh + o); }
@@ -252,6 +258,10 @@ __device__ __forceinline__ void wg_bar_sync() {                 // named barrier
 __device__ __forceinline__ void zero16(float (&d)[16]) {
 #pragma unroll
   for (int e = 0; e < 16; e++) d[e] = 0.0f;
+}
+__device__ __forceinline__ void zero16_opaque(float (&d)[16]) {
+#pragma unroll
+  for (int e = 0; e < 16; e++) asm volatile("mov.b32 %0, 0;" : "=f"(d[e])::"memory");
 }
 // columns c, c + 1 (c even) of row r of a [128 x 32] tf32 operand tile (canonical K-major, hi | lo): one 8-byte store per tile
 __device__ __forceinline__ void put2(float* hi, int r, int c, float a, float b) {
@@ -385,7 +395,7 @@ __device__ __forceinline__ void issue_fc(Issuer& I, const TileSmem& t, int half)
     if (half == 0) zero16(d); else ld_frag(p, d);
     tc::wg_fence();
 #pragma unroll
-    for (int u = 0; u < nu; u++) mma_rows<H16>(d, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c, 1);
+    for (int u = 0; u < nu; u++) mma_rows<H16, 1>(d, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c);
     tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d);
     st_frag(p, d);
   }
@@ -402,8 +412,8 @@ __device__ __forceinline__ void issue_l0(Issuer& I, const TileSmem& t, float (&d
   tc::wg_fence();
 #pragma unroll
   for (int u = 0; u < nu; u++) {
-    mma_rows<H16>(d1, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 0, 2);
-    mma_rows<H16>(d3, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 1, 2);
+    mma_rows<H16, 2>(d1, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 0);
+    mma_rows<H16, 2>(d3, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 1);
   }
   tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d1); tc::fence_acc(d3);
   release_units(I, t, nu, t.bars + B_DONE + b);
@@ -420,7 +430,7 @@ __device__ __forceinline__ void issue_h(Issuer& I, const TileSmem& t, float (&d1
     zero16(d1);
   }
   tc::wg_fence();
-  mma_rows<H16>(d1, hbuf, 0, w, 32, 32, 0, H16 ? 2 : 4);
+  mma_rows<H16, H16 ? 2 : 4>(d1, hbuf, 0, w, 32, 32, 0);
   tc::wg_commit();
 }
 
@@ -460,6 +470,7 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
     if (n >= 2) wait_group(t, n - 2);
     gather_tile<H16>(P.in.grid[0], t.a[n & 1], G.xnc, warp, lane);
     publish(t, n & 1); n++;
+    zero16_opaque(d1); zero16_opaque(d3);                        // (straight-line zeros would be materialised inside the MMA group)
     issue_l0<H16>(I, t, d1, d3);
     mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
   }
@@ -469,11 +480,10 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
   float* hbuf = t.a[n & 1];
   const int wg = threadIdx.x >> 7, q = lane & 3;
   const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);        // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8
+  float v2[16];
+  if (xyz) ld_frag(d2_frag(0), v2);
 #pragma unroll 1
   for (int i = 0; i < 5; i++) {
-    float v2[16];
-    if (xyz) ld_frag(d2_frag(i), v2);                            // (issued before the wait: the load latency hides under layer i's MMA)
-    if (i > 0) { tc::wg_wait0(); tc::fence_acc(d1); release_units(I, t, 1); }
     if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // the layer's weight slot is free: request the next units now, under the epilogue
     NSB_PH(7);
     // epilogue of layer i on the fragment: h = relu(D + b_i) + (D2_i + bc_i)
@@ -523,6 +533,10 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
     wg_bar_sync();                                               // this warpgroup's rows of H are written -> its MMA
     issue_h<H16>(I, t, d1, d3, hbuf, i + 1);
     NSB_PH(9);
+    // layer i + 1 is waited for here, on the path that issued it (a wait under `i > 0` at the top of the loop left ptxas a path on
+    // which the epilogue reads an accumulator in flight)
+    if (xyz) ld_frag(d2_frag(i + 1), v2);                        // (issued before the wait: the load latency hides under the MMA)
+    tc::wg_wait0(); tc::fence_acc(d1); release_units(I, t, 1);
   }
   NSB_PH(8);
   // output layer: per-row dot products over the fragment, summed over the four lanes of a row; handed to the row owners through this
@@ -617,14 +631,15 @@ __device__ __forceinline__ void gather_tile_kt(const nsb_grid& g, float* c_hi, i
 __device__ __forceinline__ void wg_group(WgSmem& w, int part, float* dst, int pitch, int n_rows, bool transposed3 = false) {
   fence_proxy_async();
   __syncthreads();
-  if (threadIdx.x < 128) {                                       // warpgroup 0: D[64 x 32] = [DU | G] . B^T over the 128 points
+  // warpgroup 0: D[64 x 32] = [DU | G] . B^T over the 128 points (the index comes through a shuffle: ptxas then knows the branch is
+  // warp-uniform and does not serialize the group, see mma_rows)
+  if (__shfl_sync(0xffffffffu, threadIdx.x >> 7, 0) == 0) {
     const uint64_t ah = tc::make_desc(w.du, 128u, 4096u), al = ah + (uint64_t)((kWgALo * 4) >> 4);
     const uint64_t bh = tc::make_desc(w.b, 128u, 4096u), bl = bh + (uint64_t)((kWgBLo * 4) >> 4);
     float d[16];
-#pragma unroll
-    for (int e = 0; e < 16; e++) d[e] = 0.0f;
+    zero16_opaque(d);
     tc::wg_fence();
-#pragma unroll 1
+#pragma unroll
     for (int ks = 0; ks < TM / 8; ks++) {                       // 8 points per k-step = two core matrices = 256 bytes
       const uint64_t o = 16u * (uint64_t)ks;
       tc::wgmma_tf32_n32(d, al + o, bh + o); tc::wgmma_tf32_n32(d, ah + o, bl + o); tc::wgmma_tf32_n32(d, ah + o, bh + o);
@@ -712,40 +727,48 @@ __device__ __forceinline__ void bwd_gout(const BwdExtra& X, int lv, int r, int n
 // DF += DU * W_i[:, first input] (i = 3, 0).  A layer has up to six units (fine decoder, layer 3) for the four ring slots: they go out in waves
 // of at most kSlots units, each wave committed, waited for and released at once.  A wave carries one DF chunk (accumulator fa), two at layer 0,
 // where D1 is free to take the second: more would not fit in the registers beside D1 and DC.
-__device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, int lv, int i, float (&d1)[16], float (&dc)[16], float (&fa)[16]) {
-  const bool xyz = lv != 0;
-  const int ndc = xyz ? op_cd(lv) / 32 : 0, nd1 = i >= 1 ? 1 : 0, ndf = (i == 3 || i == 0) ? op_firstp(lv) / 32 : 0;
-  const int fmax = i == 0 ? 2 : 1;                               // DF chunks per wave
-  int f0 = 0;                                                    // first DF chunk of the wave
-  int nf = min(ndf, fmax);
-  int nu = ndc + nd1 + nf;
-#pragma unroll 1
-  for (int wave = 0; nu > 0; wave++) {
-    if (nf > 0) { if (i == 0) ld_frag(d2_frag(f0), fa); else zero16(fa); }
-    if (nf > 1) ld_frag(d2_frag(f0 + 1), d1);
-    if (wave == 0) {
-      if (xyz && i == 4) zero16(dc);
-      if (nd1) zero16(d1);
-    }
+// Which MMAs a wave issues is fixed at compile time (DC: the decoder has a DC chain; NDF DF chunks; L0 = layer 0), so that every wave is one
+// straight-line MMA group (see mma_rows); only the number of DC units, ndc, which shifts the others in the ring, is a run-time value.
+template <bool DC, int NDF, bool L0>
+__device__ __forceinline__ void issue_bwd_layer_t(Issuer& I, const TileSmem& t, int ndc, float (&d1)[16], float (&dc)[16], float (&fa)[16]) {
+  constexpr int ND1 = L0 ? 0 : 1, FMAX = L0 ? 2 : 1;             // D1 units, DF chunks per wave
+  constexpr int kWaves = NDF > FMAX ? (NDF + FMAX - 1) / FMAX : 1;
+#pragma unroll
+  for (int wave = 0; wave < kWaves; wave++) {
+    const int f0 = wave * FMAX;                                  // first DF chunk of the wave
+    const int nf = NDF - f0 < FMAX ? NDF - f0 : FMAX;
+    const int k = wave == 0 ? ndc + ND1 : 0;                     // unit of the wave's first DF chunk
+    const int nu = k + nf;
 #pragma unroll 1
     for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
-    const int k = wave == 0 ? ndc + nd1 : 0;                     // unit of the wave's first DF chunk
+    if (nf > 0) { if (L0) ld_frag(d2_frag(f0), fa); else zero16_opaque(fa); }
+    if (nf > 1) ld_frag(d2_frag(f0 + 1), d1);
+    if (wave == 0 && ND1) zero16_opaque(d1);
     tc::wg_fence();
     if (wave == 0) {
-      if (xyz) mma_rows<false>(dc, t.a[0], 0, issued_unit(I, t, 0), 32, 32, 0, 4);
-      if (nd1) mma_rows<false>(d1, t.a[1], 0, issued_unit(I, t, ndc), 32, 32, 0, 4);
+      if (DC) mma_rows<false, 4>(dc, t.a[0], 0, issued_unit(I, t, 0), 32, 32, 0);
+      if (ND1) mma_rows<false, 4>(d1, t.a[1], 0, issued_unit(I, t, ndc), 32, 32, 0);
     }
-    if (nf > 0) mma_rows<false>(fa, t.a[1], 0, issued_unit(I, t, k), 32, 32, 0, 4);
-    if (nf > 1) mma_rows<false>(d1, t.a[1], 0, issued_unit(I, t, k + 1), 32, 32, 0, 4);
+    if (nf > 0) mma_rows<false, 4>(fa, t.a[1], 0, issued_unit(I, t, k), 32, 32, 0);
+    if (nf > 1) mma_rows<false, 4>(d1, t.a[1], 0, issued_unit(I, t, k + 1), 32, 32, 0);
     tc::wg_commit(); tc::wg_wait0();
     tc::fence_acc(dc); tc::fence_acc(d1); tc::fence_acc(fa);
     if (nf > 0) st_frag(d2_frag(f0), fa);
     if (nf > 1) st_frag(d2_frag(f0 + 1), d1);
     release_units(I, t, nu);
-    f0 += nf;
-    nf = min(ndf - f0, fmax);
-    nu = nf;
   }
+}
+template <bool XYZ>
+__device__ __forceinline__ void issue_bwd_layer_x(Issuer& I, const TileSmem& t, int ndc, int i, float (&d1)[16], float (&dc)[16], float (&fa)[16]) {
+  constexpr int NDF = op_firstp(XYZ ? 1 : 0) / 32;               // (the same for every xyz decoder)
+  if (XYZ && i == 4) zero16_opaque(dc);
+  if (i == 3) issue_bwd_layer_t<XYZ, NDF, false>(I, t, ndc, d1, dc, fa);
+  else if (i == 0) issue_bwd_layer_t<XYZ, NDF, true>(I, t, ndc, d1, dc, fa);
+  else issue_bwd_layer_t<XYZ, 0, false>(I, t, ndc, d1, dc, fa);
+}
+__device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, int lv, int i, float (&d1)[16], float (&dc)[16], float (&fa)[16]) {
+  if (lv != 0) issue_bwd_layer_x<true>(I, t, op_cd(lv) / 32, i, d1, dc, fa);
+  else issue_bwd_layer_x<false>(I, t, 0, i, d1, dc, fa);
 }
 
 // ---- backward of one decoder.  Leaves dL/dc rows ([128][32] fp32) in a[0] and the embedding-chain part of dL/dp ([128][4] fp32, row r at
