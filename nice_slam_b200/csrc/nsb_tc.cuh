@@ -571,7 +571,6 @@ template <typename F>
 __device__ __forceinline__ void scatter_rows(const nsb_grid& g, float* __restrict__ dgrid, const int32_t* __restrict__ slots,
                                              const float* dcs, int cd,
                                              const float xn[3], int warp, int lane, F&& emit) {
-  const bool fast = grid_fast(g);
   const int q = lane & 7, qd = warp & 3, it0 = (warp >> 2) * (8 / kCG);
 #pragma unroll 1
   for (int it = it0; it < it0 + 8 / kCG; it++) {
@@ -579,48 +578,11 @@ __device__ __forceinline__ void scatter_rows(const nsb_grid& g, float* __restric
     const int row = qd * 32 + src_lane;
     float x[3];
     x[0] = __shfl_sync(0xffffffffu, xn[0], src_lane); x[1] = __shfl_sync(0xffffffffu, xn[1], src_lane); x[2] = __shfl_sync(0xffffffffu, xn[2], src_lane);
-    const Tri t = make_tri(x, g.W, g.H, g.D);
     const float4 d4 = *reinterpret_cast<const float4*>(dcs + row * cd + 4 * q);
     const float dc[4] = {d4.x, d4.y, d4.z, d4.w};
-    float gi[3] = {0.f, 0.f, 0.f};
-    long long offs[8]; float4 vv[8]; bool ins[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {                                // all corner loads first (branch-free clamped addressing)
-      int cx, cy, cz;
-      ins[k] = tri_corner(t, k, g.W, g.H, g.D, cx, cy, cz);
-      tri_corner_clamped(t, k, g.W, g.H, g.D, cx, cy, cz);
-      offs[k] = cz * g.stride_d + cy * g.stride_h + cx * g.stride_w;
-      vv[k] = grid_load4(g, offs[k], 4 * q, fast);
-    }
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      if (ins[k]) {
-        const float4 v = vv[k];
-        const float dot = v.x * dc[0] + v.y * dc[1] + v.z * dc[2] + v.w * dc[3];
-        if (dgrid != nullptr) {
-          int cx, cy, cz;
-          tri_corner(t, k, g.W, g.H, g.D, cx, cy, cz);
-          voxel_grad_add(g, dgrid, slots, offs[k], cx, cy, cz, q, fast, tri_weight(t, k), dc);
-        }
-        const float wx = (k & 1) ? t.w1[0] : t.w0[0], wy = (k & 2) ? t.w1[1] : t.w0[1], wz = (k & 4) ? t.w1[2] : t.w0[2];
-        gi[0] += ((k & 1) ? 1.f : -1.f) * wy * wz * dot;
-        gi[1] += ((k & 2) ? 1.f : -1.f) * wx * wz * dot;
-        gi[2] += ((k & 4) ? 1.f : -1.f) * wx * wy * dot;
-      }
-    }
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-      float v = gi[a];
-      v += __shfl_xor_sync(0xffffffffu, v, 1); v += __shfl_xor_sync(0xffffffffu, v, 2); v += __shfl_xor_sync(0xffffffffu, v, 4);
-      gi[a] = v;
-    }
-    if (q == 0) {
-      const int size[3] = {g.W, g.H, g.D};
-      float gx[3];
-#pragma unroll
-      for (int a = 0; a < 3; a++) gx[a] = t.clipg[a] * ((float)(size[a] - 1) * 0.5f) * gi[a];
-      emit(row, gx);
-    }
+    float gx[3];
+    scatter_pass(g, dgrid, slots, x, dc, q, gx);
+    if (q == 0) emit(row, gx);
   }
 }
 

@@ -19,7 +19,9 @@
 // Shared memory: 64 KB activations + 40 KB ring + 6 KB headers + < 6 KB state <= 113 KB -> two CTAs per SM.
 //
 // Arithmetic is that of nsb_tc.cuh (3xTF32 split, same operand order), so results match the round-1 kernels to rounding of the output
-// layer's partial sums.
+// layer's partial sums.  Sampling and the sort, compositing and its backward, the trilinear scatter, the ray-gradient store and the
+// loss-seed / pose tails are the functions every kernel family calls from nsb_render.cu; this file keeps only the tile's mapping of
+// threads and scratch around them.
 #pragma once
 
 namespace nsb {
@@ -966,7 +968,6 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
 template <typename F>
 __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restrict__ dgrid, const int32_t* __restrict__ slots,
                                              const float* dcs, const float xn[3], int warp, int lane, F&& emit) {
-  const bool fast = grid_fast(g);
   const int q = lane & 7, qd = warp & 3, it0 = (warp >> 2) * 4;
 #pragma unroll 1
   for (int it = it0; it < it0 + 4; it++) {
@@ -974,43 +975,11 @@ __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restric
     const int row = qd * 32 + src_lane;
     float x[3];
     x[0] = __shfl_sync(0xffffffffu, xn[0], src_lane); x[1] = __shfl_sync(0xffffffffu, xn[1], src_lane); x[2] = __shfl_sync(0xffffffffu, xn[2], src_lane);
-    const Tri t = make_tri(x, g.W, g.H, g.D);
     const float4 d4 = *reinterpret_cast<const float4*>(dcs + row * 32 + 4 * q);
     const float dc[4] = {d4.x, d4.y, d4.z, d4.w};
-    float gi[3] = {0.f, 0.f, 0.f};
-    float4 vv[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      int cx, cy, cz;
-      tri_corner_clamped(t, k, g.W, g.H, g.D, cx, cy, cz);
-      vv[k] = grid_load4(g, cz * g.stride_d + cy * g.stride_h + cx * g.stride_w, 4 * q, fast);
-    }
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      int cx, cy, cz;
-      if (tri_corner(t, k, g.W, g.H, g.D, cx, cy, cz)) {         // corners outside the grid get neither gradient nor a dot product
-        const float4 v = vv[k];
-        const float dot = v.x * dc[0] + v.y * dc[1] + v.z * dc[2] + v.w * dc[3];
-        if (dgrid != nullptr) voxel_grad_add(g, dgrid, slots, cz * g.stride_d + cy * g.stride_h + cx * g.stride_w, cx, cy, cz, q, fast, tri_weight(t, k), dc);
-        const float wx = (k & 1) ? t.w1[0] : t.w0[0], wy = (k & 2) ? t.w1[1] : t.w0[1], wz = (k & 4) ? t.w1[2] : t.w0[2];
-        gi[0] += ((k & 1) ? 1.f : -1.f) * wy * wz * dot;
-        gi[1] += ((k & 2) ? 1.f : -1.f) * wx * wz * dot;
-        gi[2] += ((k & 4) ? 1.f : -1.f) * wx * wy * dot;
-      }
-    }
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-      float v = gi[a];
-      v += __shfl_xor_sync(0xffffffffu, v, 1); v += __shfl_xor_sync(0xffffffffu, v, 2); v += __shfl_xor_sync(0xffffffffu, v, 4);
-      gi[a] = v;
-    }
-    if (q == 0) {
-      const int size[3] = {g.W, g.H, g.D};
-      float gx[3];
-#pragma unroll
-      for (int a = 0; a < 3; a++) gx[a] = t.clipg[a] * ((float)(size[a] - 1) * 0.5f) * gi[a];
-      emit(row, gx);
-    }
+    float gx[3];
+    scatter_pass(g, dgrid, slots, x, dc, q, gx);
+    if (q == 0) emit(row, gx);
   }
 }
 
@@ -1065,22 +1034,7 @@ __device__ __forceinline__ void composite_ray(const KParams& P, int ray, int lan
     *reinterpret_cast<float4*>(P.fo.raw + 4 * (g0 + s)) = v;
   }
   __syncwarp();
-  ray_weights(rw, S, lane, wq, nullptr);
-  __syncwarp();
-  float c0 = 0.f, c1 = 0.f, c2 = 0.f; double dsum = 0.0;
-  for (int s = lane; s < S; s += 32) {
-    const float w = wq[s];
-    c0 = fmaf(w, rw[4 * s], c0); c1 = fmaf(w, rw[4 * s + 1], c1); c2 = fmaf(w, rw[4 * s + 2], c2);
-    dsum += (double)w * zz[s];
-  }
-  c0 = warp_sum(c0); c1 = warp_sum(c1); c2 = warp_sum(c2); dsum = warp_sum(dsum);
-  double v = 0.0;
-  for (int s = lane; s < S; s += 32) { const double tt = zz[s] - dsum; v += (double)wq[s] * tt * tt; }
-  v = warp_sum(v);
-  if (lane == 0) {
-    P.fo.depth[ray] = dsum; P.fo.var[ray] = v;
-    P.fo.rgb[3 * ray] = c0; P.fo.rgb[3 * ray + 1] = c1; P.fo.rgb[3 * ray + 2] = c2;
-  }
+  composite_ray_outputs(P, ray, rw, zz, wq, lane);
   __syncwarp();
 }
 
@@ -1096,7 +1050,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int row = tid & (TM - 1), cg = tid >> 7;            // (control warp: row/cg unused)
   TileSmem t; carve(smem_raw, t, false);
-  __shared__ int s_ndone, s_done[kMaxTileRays], s_last;
+  __shared__ int s_ndone, s_done[kMaxTileRays];
   __shared__ float s_max[16];
   __shared__ uint32_t s_seq;
 
@@ -1132,80 +1086,18 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
     make_point_from_p(P.in.bound, P.in.coarse_bound, pin, G);
     __syncthreads();
   } else {
-    float gtmax = 0.0f, gtmax12 = 0.0f;
-    if (P.has_gt) {
-      if (P.in.depth_max != nullptr) { gtmax = P.in.depth_max[0]; gtmax12 = P.in.depth_max[1]; }
-      else {                                                      // small batches: every CTA reduces the sensor depths itself (Renderer.py:109,144)
-        const bool whole = P.in.gt_depth_batch != nullptr;        // the depths of the whole (sharded) batch are known here: no exchange
-        const float* gsrc = whole ? P.in.gt_depth_batch : P.in.gt_depth;
-        const int gn = whole ? P.in.n_batch : P.in.n_rays;
-        float m = -INFINITY;
-        for (int i = tid; i < gn; i += kThreads) m = fmaxf(m, __ldg(gsrc + i));
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        if (lane == 0) s_max[warp] = m;
-        __syncthreads();
-        m = -INFINITY;
-        for (int w = 0; w < kThreads / 32; w++) m = fmaxf(m, s_max[w]);
-        if (P.fs.px.world > 1 && !whole) m = peer_max_all_ctas(P.fs.px, m, &s_seq);      // sharded batch: MAX over the ranks' shards (Renderer.py:109,144)
-        gtmax = m; gtmax12 = __fmul_rn(m, 1.2f);
-      }
-    }
+    float gtmax, gtmax12;
+    batch_depth_max(P, s_max, &s_seq, gtmax, gtmax12);
     NSB_PH(40);
-    // scratch in the (still unused) operand buffers: ray table [nr][8] f32 + far [nr] f64 | unsorted z [nr*S] | sorted z [nr*S]
+    // scratch in the (still unused) operand buffers: ray table [nr][8] f32 + far [nr] f64 | unsorted z [nr*S] | sorted z [nr*S] | flags [nr]
     float* rays = t.a[0];
     double* far = reinterpret_cast<double*>(t.a[0] + 8 * kMaxTileRays);
     double* zu = far + kMaxTileRays;
     double* zs = zu + (size_t)nr * S;
-    for (int r = tid; r < nr; r += kThreads) {
-      float o[3], d[3];
-#pragma unroll
-      for (int a = 0; a < 3; a++) { o[a] = P.in.rays_o[3 * (ray_lo + r) + a]; d[a] = P.in.rays_d[3 * (ray_lo + r) + a]; }
-      const float gt = P.has_gt ? P.in.gt_depth[ray_lo + r] : 0.0f;
-      const RaySampler rs = make_sampler(P.in.bound, o, d, P.has_gt, gt, gtmax12);
-#pragma unroll
-      for (int a = 0; a < 3; a++) { rays[8 * r + a] = o[a]; rays[8 * r + 3 + a] = d[a]; }
-      rays[8 * r + 6] = rs.near; rays[8 * r + 7] = gt; far[r] = rs.far;
-    }
+    block_setup_rays(P, rays, far, ray_lo, nr, gtmax12);
     __syncthreads();
     NSB_PH(41);
-    for (int i = tid; i < nr * S; i += kThreads) {
-      const int r = i / S, s = i - r * S;
-      RaySampler rs; rs.near = rays[8 * r + 6]; rs.gt = rays[8 * r + 7]; rs.far = far[r]; rs.has_gt = P.has_gt;
-      zu[i] = sample_z(rs, s, P.in.n_samples, P.in.t_uniform, P.in.t_surface, gtmax);
-    }
-    __syncthreads();
-    NSB_PH(42);
-    // torch.sort of the concatenation [uniform | surface] (Renderer.py:168-170).  Both lists come out of linspace-style formulas and are
-    // normally non-decreasing: then the stable rank of an element is its index in its own list plus a binary-search count in the other one
-    // (merge by ranks).  A ray whose lists are not sorted (far < near, NaN) takes the general stable rank sort -- same values either way.
-    int* unsorted = reinterpret_cast<int*>(zs + (size_t)nr * S);
-    for (int r = tid; r < nr; r += kThreads) unsorted[r] = 0;
-    __syncthreads();
-    const int nu = P.in.n_samples < S ? P.in.n_samples : S;
-    for (int i = tid; i < nr * S; i += kThreads) {
-      const int r = i / S, s = i - r * S;
-      if (s != 0 && s != nu) { const double a = zu[i - 1], b = zu[i]; if (!(a <= b)) unsorted[r] = 1; }
-      else if (zu[i] != zu[i]) unsorted[r] = 1;
-    }
-    __syncthreads();
-    for (int i = tid; i < nr * S; i += kThreads) {
-      const int r = i / S, s = i - r * S;
-      const double zi = zu[i];
-      const double* zr = zu + r * S;
-      int rank;
-      if (!unsorted[r]) {
-        // uniform element: + #{surface < z}; surface element: + #{uniform <= z} (cat order = uniform first, stable)
-        const bool uni = s < nu;
-        const double* other = uni ? zr + nu : zr;
-        int lo = 0, hi = uni ? S - nu : nu;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; const double zm = other[mid]; if (uni ? (zm < zi) : (zm <= zi)) lo = mid + 1; else hi = mid; }
-        rank = (uni ? s : s - nu) + lo;
-      } else {
-        rank = 0;
-        for (int j = 0; j < S; j++) { const double zj = zr[j]; rank += (z_less(zj, zi) || (!z_less(zi, zj) && j < s)) ? 1 : 0; }
-      }
-      zs[r * S + rank] = zi;
-    }
+    block_sample_sort(P, rays, far, nr, gtmax, zu, zs, reinterpret_cast<int*>(zs + (size_t)nr * S));
     __syncthreads();
     NSB_PH(43);
     {
@@ -1258,17 +1150,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   NSB_PH(15);
   for (int k = warp; k < nd; k += kThreads / 32) composite_ray(P, s_done[k], lane, smem_raw + (size_t)warp * composite_scratch_bytes(S));
   NSB_PH(16);
-  // loss seeds: the last CTA of the grid to get here sees every ray composited
-  if (P.fs.kind != 0 && grid_last_arrival(P.fs.counter, gridDim.x, &s_last)) {
-    if (P.fs.kind == 1) {
-      tracking_seeds_body(P.fo.depth, P.fo.var, P.fo.rgb, P.in.gt_depth, static_cast<const double*>(P.fs.gt_rgb), P.in.n_rays, P.fs.w_color,
-                          P.fs.handle_dynamic, P.fs.use_color, nullptr, 0, P.fs.g_depth, P.fs.g_rgb, P.fs.loss, P.fs.res, P.fs.px, smem_raw);
-      if (P.fs.px.world > 1 && P.in.depth_max == nullptr && P.in.gt_depth_batch == nullptr && tid == 0) peer_advance(P.fs.px, 0);      // every CTA is past the depth-max exchange
-    } else {
-      mapping_seeds_body(P.fo.depth, P.fo.rgb, P.fs.gt_depth_loss, static_cast<const float*>(P.fs.gt_rgb), P.in.n_rays, P.fs.w_color, P.fs.use_color,
-                         P.fs.g_depth, P.fs.g_rgb, P.fs.loss, smem_raw);
-    }
-  }
+  fused_seeds_tail(P, gridDim.x, smem_raw);                       // the last CTA of the grid to get here sees every ray composited
 }
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false>(P); }
 // forward with FP16 hi|lo operands (option fwd_f16; see mma_rows)
@@ -1329,48 +1211,19 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
     for (int a = 0; a < 3; a++) { o[a] = P.in.rays_o[3 * ray + a]; d[a] = P.in.rays_d[3 * ray + a]; }
     for (int s = lane; s < S; s += 32) *reinterpret_cast<float4*>(rw + 4 * s) = *reinterpret_cast<const float4*>(P.bw.raw + 4 * (g0 + s));
     __syncwarp();
-    const double gD = P.bw.g_depth != nullptr ? P.bw.g_depth[ray] : 0.0;
-    const double gV = P.bw.g_var != nullptr ? P.bw.g_var[ray] : 0.0;
     float g3[3] = {0.f, 0.f, 0.f};
     if (P.bw.g_rgb != nullptr) { g3[0] = P.bw.g_rgb[3 * ray]; g3[1] = P.bw.g_rgb[3 * ray + 1]; g3[2] = P.bw.g_rgb[3 * ray + 2]; }
     if (lane == 0) { X.gc[3 * r] = g3[0]; X.gc[3 * r + 1] = g3[1]; X.gc[3 * r + 2] = g3[2]; }
-    ray_weights(rw, S, lane, wq, go);                            // go[] temporarily holds T_s
-    __syncwarp();
     const double* z = P.bw.z_vals + g0;
-    double Dm = 0.0;
-    for (int s = lane; s < S; s += 32) Dm += (double)wq[s] * z[s];
-    Dm = warp_sum(Dm);
-    double swt = 0.0;
-    for (int s = lane; s < S; s += 32) swt += (double)wq[s] * (z[s] - Dm);
-    swt = warp_sum(swt);
-    const double gDe = gD + gV * (-2.0 * swt);
-    float carry = 0.0f;
-    const int nblk = (S + 31) / 32;
-    for (int b = nblk - 1; b >= 0; b--) {
-      const int s = b * 32 + lane;
-      const bool v = s < S;
-      float gw = 0.0f, al = 0.0f, T = 0.0f, w = 0.0f;
-      if (v) {
-        al = sigmoid_f(10.0f * rw[4 * s + 3]); T = go[s]; w = wq[s];
-        const double tt = z[s] - Dm;
-        gw = (float)(gDe * z[s] + gV * tt * tt) + g3[0] * rw[4 * s] + g3[1] * rw[4 * s + 1] + g3[2] * rw[4 * s + 2];
+    composite_ray_backward(rw, z, S, P.bw.g_depth != nullptr ? P.bw.g_depth[ray] : 0.0, P.bw.g_var != nullptr ? P.bw.g_var[ray] : 0.0, g3,
+                           wq, go, lane, [&](int s, float w, float al, float ga) {
+      const long long gp = g0 + s;
+      if (gp >= gp0 && gp < gp0 + npts) {                          // only the samples of this tile are needed
+        PointGeom Gs; make_point(P.in.bound, P.in.coarse_bound, o, d, z[s], Gs);
+        X.gocc[gp - gp0] = Gs.inb ? 10.0f * al * (1.0f - al) * ga : 0.0f;
+        X.wgt[gp - gp0] = w;
       }
-      const float incl = warp_incl_suffix_sum(gw * w, lane);
-      float excl = __shfl_down_sync(0xffffffffu, incl, 1);
-      if (lane == 31) excl = 0.0f;
-      const float R = carry + excl;
-      if (v) {
-        const long long gp = g0 + s;
-        if (gp >= gp0 && gp < gp0 + npts) {                      // only the samples of this tile are needed
-          PointGeom Gs; make_point(P.in.bound, P.in.coarse_bound, o, d, z[s], Gs);
-          const float qd = (1.0f - al) + 1e-10f;
-          const float ga = T * gw - R / qd;
-          X.gocc[gp - gp0] = Gs.inb ? 10.0f * al * (1.0f - al) * ga : 0.0f;
-          X.wgt[gp - gp0] = w;
-        }
-      }
-      carry += __shfl_sync(0xffffffffu, incl, 0);
-    }
+    });
   }
   NSB_PH(20);
   PointGeom G;
@@ -1443,24 +1296,10 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
         so += __ldcg(pp + a); sd += __ldcg(pp + 3 + a);
       }
     }
-    if (P.accumulate_rays) {
-      if (P.bw.d_rays_o != nullptr) so += (double)P.bw.d_rays_o[3 * ray + a];
-      if (P.bw.d_rays_d != nullptr) sd += (double)P.bw.d_rays_d[3 * ray + a];
-    }
-    if (P.bw.d_rays_o != nullptr) P.bw.d_rays_o[3 * ray + a] = (float)so;
-    if (P.bw.d_rays_d != nullptr) P.bw.d_rays_d[3 * ray + a] = (float)sd;
+    store_ray_grad(P, ray, a, so, sd);
   }
   NSB_PH(32);
-  if (fused_pose_grad(P, gridDim.x, reinterpret_cast<double*>(smem_raw)) && P.tail.px.world > 1) {
-    // sharded tracking batch: SUM over ranks of [loss | d c2w] by this (last) CTA -- identical bits on every rank
-    __shared__ double tot[13];
-    __shared__ uint32_t s_seq2;
-    __syncthreads();
-    if (tid == 0) tot[0] = P.tail.loss != nullptr ? P.tail.loss[0] : 0.0;
-    if (tid < 12) tot[1 + tid] = P.bw.d_c2w[tid];
-    __syncthreads();
-    peer_sum13(P.tail.px, tot, 13, P.tail.out13, &s_seq2);
-  }
+  if (fused_pose_grad(P, gridDim.x, reinterpret_cast<double*>(smem_raw))) pose_tail_peers(P);
 }
 __global__ void __launch_bounds__(tl::kThreads, 2) render_bwd_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<false>(P); }
 __global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<true>(P); }

@@ -14,7 +14,7 @@ from gpu_util import make_renderer  # noqa: E402
 from nice_slam_b200 import _lib  # noqa: E402
 from nice_slam_b200.steps import IterationContext  # noqa: E402
 
-TILE_NAMES = {40: "fwd: launch -> depth max done", 41: "fwd: ray table (bbox far, near)", 42: "fwd: sample z", 43: "fwd: rank sort", 44: "fwd: point geometry + syncs",
+TILE_NAMES = {40: "fwd: launch -> depth max done", 41: "fwd: ray table (bbox far, near)", 43: "fwd: sample z + rank sort", 44: "fwd: point geometry + syncs",
               1: "fwd: gather (per grid)", 2: "fwd: publish + issue fc_c", 6: "fwd: wait free buffer (E block)", 3: "fwd: embed block compute", 4: "fwd: publish + issue layer-0 block",
               7: "fwd: wait MMAs of the layer", 8: "fwd: layer epilogue (relu, masks, H write)", 9: "fwd: publish + issue hidden layer", 12: "fwd: output layer + syncs",
               14: "fwd: dealloc + sync", 15: "fwd: parts store + ray completion", 16: "fwd: compositing of completed rays",
