@@ -182,6 +182,35 @@ size_t nsb_backward_workspace_bytes(void);
 /* Backward of the same path (what loss.backward() does at src/Tracker.py:125 / src/Mapper.py:503). */
 int nsb_render_backward(const nsb_render_inputs* in, const nsb_backward_args* bw, void* stream);
 
+/* ---- the other sampling settings of the reference's `rendering:` block (src/utils/Renderer.py:152-166, 181-196) ----------------------
+ * nsb_render_forward / nsb_render_backward are nsb_render_forward_sampled / nsb_render_backward_sampled with sampling == NULL.
+ *   lindisp   != 0: the stratified samples are spaced in inverse depth, z = 1/(1/near (1-t) + 1/far t)  (Renderer.py:154-157;
+ *             1/near (1-t) float32, the rest float64, as the reference's dtypes; a ray with gt_depth 0 gets z = 0 and z = NaN at t = 1)
+ *   t_rand    device f32 [N, n_samples] or NULL: perturb > 0, the uniforms of torch.rand(z_vals.shape) (Renderer.py:159-166): sample i
+ *             moves to lower_i + (upper_i - lower_i) t_rand[i] inside the interval between the midpoints of its neighbours
+ *   z_vals    device f64 [N, S] or NULL: render this sorted sample list instead of sampling (the second pass of hierarchical sampling,
+ *             Renderer.py:181-196, z_vals from nsb_importance_samples); lindisp / t_rand are then ignored and S <= NSB_MAX_SAMPLES
+ *             replaces n_samples + n_surface as the samples per ray.  The backward takes its forward's nsb_sampling (only S is used). */
+typedef struct {
+  int32_t lindisp;
+  const float* t_rand;
+  const double* z_vals;
+  int32_t S;
+} nsb_sampling;
+
+/* Forward with the sampling settings above (Renderer.render_batch_ray, src/utils/Renderer.py:63-198). */
+int nsb_render_forward_sampled(const nsb_render_inputs* in, const nsb_sampling* sampling, const nsb_forward_outputs* out, void* stream);
+/* Backward of nsb_render_forward_sampled (src/Tracker.py:125 / src/Mapper.py:503); z comes from bw->z_vals. */
+int nsb_render_backward_sampled(const nsb_render_inputs* in, const nsb_sampling* sampling, const nsb_backward_args* bw, void* stream);
+/* Hierarchical importance sampling (Renderer.py:181-185, sample_pdf src/common.py:19-63) for a first pass of S0 samples per ray:
+ * from its sorted z_vals [N,S0] (f64) and raw [N,S0,4] (nsb_forward_outputs.raw), the compositing weights w, then
+ * sample_pdf(bins = mid-points of z_vals, w[1:-1], n_importance): +1e-5, normalise, cumsum, searchsorted(right=True), lerp
+ * (weights / cdf float32, bins and samples float64).  u: device f32, [n_importance] (u_per_ray == 0: torch.linspace(0,1,n_importance),
+ * the reference's perturb == 0) or [N, n_importance] (u_per_ray != 0: torch.rand).  z_out [N, S0 + n_importance] = torch.sort of the
+ * concatenation [z_vals | samples] (Renderer.py:185), the sample list of the second pass.  S0 >= 3, S0 + n_importance <= NSB_MAX_SAMPLES. */
+int nsb_importance_samples(const double* z_vals, const float* raw, int n_rays, int S0, int n_importance, const float* u, int u_per_ray,
+                           double* z_out, void* stream);
+
 /* Loss seeds.  Tracking (src/Tracker.py:108-123): residual r = |gt-depth|/sqrt(var+1e-10), mask =
  * (r < 10*median(r)) & (gt>0) when handle_dynamic else gt>0; loss = sum_mask r + w_color*sum_mask|gt_rgb-rgb|.
  * Mapping (src/Mapper.py:487-493): loss = sum_{gt>0}|gt-depth| (+ w_color*sum|gt_rgb-rgb| in stage color).

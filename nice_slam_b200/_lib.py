@@ -54,6 +54,10 @@ class BackwardArgs(C.Structure):
                 ("result_dst", C.c_void_p), ("result_src", C.c_void_p), ("result_bytes", C.c_size_t)]
 
 
+class Sampling(C.Structure):
+    _fields_ = [("lindisp", C.c_int32), ("t_rand", C.c_void_p), ("z_vals", C.c_void_p), ("S", C.c_int32)]
+
+
 class IterationBuffers(C.Structure):
     _fields_ = [("depth", C.c_void_p), ("var", C.c_void_p), ("rgb", C.c_void_p), ("z_vals", C.c_void_p), ("raw", C.c_void_p),
                 ("masks", C.c_void_p), ("g_depth", C.c_void_p), ("g_rgb", C.c_void_p), ("loss", C.c_void_p), ("depth_max", C.c_void_p),
@@ -79,6 +83,9 @@ SYMBOLS = {
     "nsb_batch_max_depth": (C.c_int, [_P, C.c_int, _P, _P]),
     "nsb_bbox_prefilter": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_double), _P, _P]),
     "nsb_render_forward": (C.c_int, [C.POINTER(RenderInputs), C.POINTER(ForwardOutputs), _P]),
+    "nsb_render_forward_sampled": (C.c_int, [C.POINTER(RenderInputs), C.POINTER(Sampling), C.POINTER(ForwardOutputs), _P]),
+    "nsb_render_backward_sampled": (C.c_int, [C.POINTER(RenderInputs), C.POINTER(Sampling), C.POINTER(BackwardArgs), _P]),
+    "nsb_importance_samples": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "nsb_backward_workspace_bytes": (C.c_size_t, []),
     "nsb_render_backward": (C.c_int, [C.POINTER(RenderInputs), C.POINTER(BackwardArgs), _P]),
     "nsb_tracking_seeds": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),

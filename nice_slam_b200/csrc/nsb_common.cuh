@@ -207,10 +207,13 @@ struct FusedSeeds {
   int* counter;                  // grid-wide arrival counter, zero between launches
   PeerX px;                      // world > 1: sharded tracking batch -- depth maxima and the median pool are exchanged inside the forward launch
 };
-int render_forward_fused(const nsb_render_inputs* in, const nsb_forward_outputs* out, const FusedSeeds* fs, void* stream);
+// smp: nsb_sampling of the *_sampled entry points (NULL: the default sampler)
+int render_forward_fused(const nsb_render_inputs* in, const nsb_forward_outputs* out, const FusedSeeds* fs, void* stream,
+                         const nsb_sampling* smp = nullptr);
 // after_forward: the forward launch of the same iteration is the operation right in front of this call on `stream` -> the backward launch may
 // start early (programmatic dependent launch) and run its set-up under the forward's tail
-int render_backward_tail(const nsb_render_inputs* in, const nsb_backward_args* bw, const PeerTail* tail, void* stream, bool after_forward = false);
+int render_backward_tail(const nsb_render_inputs* in, const nsb_backward_args* bw, const PeerTail* tail, void* stream, bool after_forward = false,
+                         const nsb_sampling* smp = nullptr);
 int make_peerx(const struct nsb_peers* p, PeerX* px);
 
 // error plumbing shared by the API translation units

@@ -46,20 +46,33 @@ __device__ __forceinline__ RaySampler make_sampler(const double* bound, const fl
   } else { rs.near = 0.01f; rs.far = far_bb; }
   return rs;
 }
-// unsorted sample i of the concatenation [uniform(n_samples) | surface(n_surface)]
+// stratified sample at t = linspace value (Renderer.py:154-157).  lindisp: 1/near is the f32 reciprocal (near = gt*0.01 f32; the
+// Python 0.01 without sensor depth gives the same 100.0f), 1/far and the rest f64; gt = 0 gives 1/near = inf -> z = 0, and NaN at t = 1.
+__device__ __forceinline__ double uniform_z(const RaySampler& rs, float t, int lindisp) {
+  if (!lindisp) {
+    const float a = __fmul_rn(rs.near, __fsub_rn(1.0f, t));        // f32 (Renderer.py:155)
+    return __dadd_rn((double)a, __dmul_rn(rs.far, (double)t));     // f64
+  }
+  const float a = __fmul_rn(__frcp_rn(rs.near), __fsub_rn(1.0f, t));                       // f32 (:157)
+  return __drcp_rn(__dadd_rn((double)a, __dmul_rn(__drcp_rn(rs.far), (double)t)));          // f64
+}
+// unsorted sample i of the concatenation [uniform(n_samples) | surface(n_surface)] (perturb: jitter_z afterwards)
 __device__ __forceinline__ double sample_z(const RaySampler& rs, int i, int n_samples,
                                            const float* __restrict__ t_uniform, const double* __restrict__ t_surface,
-                                           float gtmax) {
-  if (i < n_samples) {
-    const float t = t_uniform[i];
-    const float a = __fmul_rn(rs.near, __fsub_rn(1.0f, t));          // f32 (Renderer.py:155)
-    return __dadd_rn((double)a, __dmul_rn(rs.far, (double)t));       // f64
-  }
+                                           float gtmax, int lindisp) {
+  if (i < n_samples) return uniform_z(rs, t_uniform[i], lindisp);
   const double ts = t_surface[i - n_samples];
   const double omt = __dsub_rn(1.0, ts);
   if (rs.gt > 0.0f)                                                  // Renderer.py:128-140
     return __dadd_rn(__dmul_rn((double)__fmul_rn(0.95f, rs.gt), omt), __dmul_rn((double)__fmul_rn(1.05f, rs.gt), ts));
   return __dadd_rn(__dmul_rn(0.001, omt), __dmul_rn((double)gtmax, ts));   // :143-150
+}
+// perturb (Renderer.py:159-166): stratified sample i of z [n] moves to lower + (upper - lower) t_rand, lower / upper = the mid-points
+// .5 (z[i-1] + z[i]) and .5 (z[i] + z[i+1]) (z[0] / z[n-1] at the ends); t_rand is promoted to f64
+__device__ __forceinline__ double jitter_z(const double* z, int i, int n, float t_rand) {
+  const double lo = i > 0 ? __dmul_rn(0.5, __dadd_rn(z[i], z[i - 1])) : z[i];
+  const double hi = i + 1 < n ? __dmul_rn(0.5, __dadd_rn(z[i + 1], z[i])) : z[i];
+  return __dadd_rn(lo, __dmul_rn(__dsub_rn(hi, lo), (double)t_rand));
 }
 // strict-weak order used by the rank sort: ascending, NaN last (torch.sort)
 __device__ __forceinline__ bool z_less(double a, double b) { return (a < b) || (b != b && a == a); }

@@ -169,6 +169,7 @@ struct KParams {
   int acts_lv;                  // forward: decoder level whose layer outputs go to fo.acts (-1: none)
   int wbytes;                   // bytes reserved for the weight image in shared memory
   int max_pts, max_rays;        // per-CTA capacities the shared-memory carve-up was sized for
+  nsb_sampling smp;             // lindisp / perturb uniforms / a given sorted z list (all zero: the default sampler)
 };
 
 struct Smem {                   // carve-up of dynamic shared memory (all offsets 16-byte aligned)
@@ -230,23 +231,37 @@ __device__ __forceinline__ void block_setup_rays(const KParams& P, float* rays, 
   }
 }
 
-// Stratified + near-surface samples of the nr rays of a ray table (block_setup_rays; call after a __syncthreads()) -> zu [nr][S], then
-// their torch.sort of [uniform | surface] (Renderer.py:82-170) -> zs [nr][S].  unsorted: [nr] per-ray flags.  Ends without a barrier.
-__device__ __forceinline__ void block_sample_sort(const KParams& P, const float* rays, const double* far, int nr, float gtmax,
+// Stratified + near-surface samples of the nr rays [r0, r0 + nr) of a ray table (block_setup_rays; call after a __syncthreads()) -> zu [nr][S],
+// then their torch.sort of [uniform | surface] (Renderer.py:82-170) -> zs [nr][S].  unsorted: [nr] per-ray flags.  A given sorted list
+// (P.smp.z_vals: the second pass of hierarchical sampling) takes the place of the uniform list.  Ends without a barrier.
+// kSampled = false compiles the default sampler only (P.smp is not read): the tile forward keeps a separate instantiation for P.smp.
+template <bool kSampled = true>
+__device__ __forceinline__ void block_sample_sort(const KParams& P, const float* rays, const double* far, int r0, int nr, float gtmax,
                                                   double* zu, double* zs, int* unsorted) {
   const int S = P.S;
   for (int i = threadIdx.x; i < nr * S; i += blockDim.x) {
     const int r = i / S, s = i - r * S;
     RaySampler rs; rs.near = rays[8 * r + 6]; rs.gt = rays[8 * r + 7]; rs.far = far[r]; rs.has_gt = P.has_gt;
-    zu[i] = sample_z(rs, s, P.in.n_samples, P.in.t_uniform, P.in.t_surface, gtmax);
+    zu[i] = kSampled && P.smp.z_vals != nullptr ? P.smp.z_vals[(long long)r0 * S + i]
+                                                : sample_z(rs, s, P.in.n_samples, P.in.t_uniform, P.in.t_surface, gtmax, kSampled ? P.smp.lindisp : 0);
   }
   __syncthreads();
+  if (kSampled && P.smp.t_rand != nullptr) {                                 // perturb: jitter the stratified samples (zs is free until the sort)
+    const int n = P.in.n_samples;
+    for (int i = threadIdx.x; i < nr * S; i += blockDim.x) {
+      const int r = i / S, s = i - r * S;
+      if (s < n) zs[i] = jitter_z(zu + r * S, s, n, P.smp.t_rand[(long long)(r0 + r) * n + s]);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < nr * S; i += blockDim.x) if (i % S < n) zu[i] = zs[i];
+    __syncthreads();
+  }
   // Both lists come out of linspace-style formulas and are normally non-decreasing: then the stable rank of an element is its index in its
   // own list plus a binary-search count in the other one (merge by ranks).  A ray whose lists are not sorted (far < near, NaN) takes the
   // general stable rank sort -- same values either way.
   for (int r = threadIdx.x; r < nr; r += blockDim.x) unsorted[r] = 0;
   __syncthreads();
-  const int nu = P.in.n_samples < S ? P.in.n_samples : S;
+  const int nu = P.in.n_samples < S && !(kSampled && P.smp.z_vals != nullptr) ? P.in.n_samples : S;
   for (int i = threadIdx.x; i < nr * S; i += blockDim.x) {
     const int r = i / S, s = i - r * S;
     if (s != 0 && s != nu) { if (!(zu[i - 1] <= zu[i])) unsorted[r] = 1; }
@@ -468,7 +483,7 @@ __device__ __forceinline__ void fwd_sample_sort(const KParams& P, const Smem& sm
     batch_depth_max(P, s_max, &s_seq, gtmax, gtmax12);
     block_setup_rays(P, sm.rays, sm.far, b.r0, b.nr, gtmax12);
     __syncthreads();
-    block_sample_sort(P, sm.rays, sm.far, b.nr, gtmax, reinterpret_cast<double*>(sm.raw), sm.zs, s_unsorted);   // (raw is not live yet)
+    block_sample_sort(P, sm.rays, sm.far, b.r0, b.nr, gtmax, reinterpret_cast<double*>(sm.raw), sm.zs, s_unsorted);   // (raw is not live yet)
   }
   __syncthreads();
   for (int lp = threadIdx.x; lp < b.Pb; lp += blockDim.x) { sm.raw[4 * lp] = 0.f; sm.raw[4 * lp + 1] = 0.f; sm.raw[4 * lp + 2] = 0.f; sm.raw[4 * lp + 3] = 0.f; }
@@ -944,6 +959,84 @@ __global__ void __launch_bounds__(tc::kThreads, 1) render_bwd_tc_kernel(const __
   NSB_PH(30);
 }
 
+// ------------------------------------------------------------------------------------------------
+// hierarchical importance sampling (Renderer.py:181-185, sample_pdf src/common.py:19-63), one warp per ray: the first pass's weights ->
+// n_importance samples of their piecewise-constant pdf over the mid-points of z -> stable sort of [z | samples] into the second pass's list
+// ------------------------------------------------------------------------------------------------
+constexpr int kImpWarps = 4;
+__global__ void __launch_bounds__(kImpWarps * 32) importance_kernel(const double* __restrict__ z_vals, const float* __restrict__ raw, int n_rays,
+                                                                    int S0, int ni, const float* __restrict__ u, int u_per_ray,
+                                                                    double* __restrict__ z_out) {
+  __shared__ float s_w[kImpWarps][NSB_MAX_SAMPLES];              // compositing weights
+  __shared__ float s_cdf[kImpWarps][NSB_MAX_SAMPLES];
+  __shared__ double s_smp[kImpWarps][NSB_MAX_SAMPLES];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ray = blockIdx.x * kImpWarps + warp;
+  if (ray >= n_rays) return;                                     // (warp-uniform; no CTA barrier below)
+  const double* z = z_vals + (long long)ray * S0;
+  float* w = s_w[warp];
+  float* cdf = s_cdf[warp];
+  double* smp = s_smp[warp];
+  ray_weights(raw + (long long)ray * S0 * 4, S0, lane, w, nullptr);
+  __syncwarp();
+  // pdf = (w[1:-1] + 1e-5) / sum, cdf = [0 | cumsum(pdf)]: float32 values; the sum and the running sum accumulate in float64 and are rounded
+  // once, as torch's CPU cumsum does (its sum associates differently: the last bit of the f32 total may differ)
+  const int M = S0 - 2;
+  double tot = 0.0;
+  for (int k = lane; k < M; k += 32) tot += (double)__fadd_rn(w[k + 1], 1e-5f);
+  const float fsum = (float)warp_sum(tot);
+  double carry = 0.0;
+  for (int base = 0; base < M; base += 32) {
+    const int k = base + lane;
+    double v = k < M ? (double)__fdiv_rn(__fadd_rn(w[k + 1], 1e-5f), fsum) : 0.0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+    if (k < M) cdf[k + 1] = (float)(carry + v);
+    carry += __shfl_sync(0xffffffffu, v, 31);
+  }
+  if (lane == 0) cdf[0] = 0.0f;
+  __syncwarp();
+  // invert the cdf: searchsorted(cdf, u, right=True), clamp, gather, lerp between the bins (mid-points of z, f64)
+  for (int j = lane; j < ni; j += 32) {
+    const float uj = u_per_ray ? u[(long long)ray * ni + j] : u[j];
+    int lo = 0, hi = M + 1;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (cdf[mid] <= uj) lo = mid + 1; else hi = mid; }
+    const int below = lo - 1 > 0 ? lo - 1 : 0, above = lo < M ? lo : M;
+    const float c0 = cdf[below];
+    float den = __fsub_rn(cdf[above], c0);
+    if (den < 1e-5f) den = 1.0f;
+    const float t = __fdiv_rn(__fsub_rn(uj, c0), den);
+    const double b0 = __dmul_rn(0.5, __dadd_rn(z[below + 1], z[below])), b1 = __dmul_rn(0.5, __dadd_rn(z[above + 1], z[above]));
+    smp[j] = __dadd_rn(b0, __dmul_rn((double)t, __dsub_rn(b1, b0)));
+  }
+  __syncwarp();
+  // torch.sort([z | samples]) by stable ranks: a merge when both lists are sorted and NaN-free (deterministic u), else the general rank sort
+  bool bad = false;
+  for (int i = lane; i < S0; i += 32) bad |= z[i] != z[i] || (i > 0 && !(z[i - 1] <= z[i]));
+  for (int j = lane; j < ni; j += 32) bad |= smp[j] != smp[j] || (j > 0 && !(smp[j - 1] <= smp[j]));
+  const bool unsorted = __any_sync(0xffffffffu, bad);
+  const int S = S0 + ni;
+  double* zo = z_out + (long long)ray * S;
+  for (int i = lane; i < S; i += 32) {
+    const bool first = i < S0;
+    const double zi = first ? z[i] : smp[i - S0];
+    int rank;
+    if (!unsorted) {                                             // z element: + #{samples < z}; sample: + #{z <= sample} (z first, stable)
+      const double* other = first ? smp : z;
+      int lo = 0, hi = first ? ni : S0;
+      while (lo < hi) { const int mid = (lo + hi) >> 1; const double zm = other[mid]; if (first ? (zm < zi) : (zm <= zi)) lo = mid + 1; else hi = mid; }
+      rank = (first ? i : i - S0) + lo;
+    } else {
+      rank = 0;
+      for (int k = 0; k < S; k++) {
+        const double zk = k < S0 ? z[k] : smp[k - S0];
+        rank += (z_less(zk, zi) || (!z_less(zi, zk) && k < i)) ? 1 : 0;
+      }
+    }
+    zo[rank] = zi;
+  }
+}
+
 }  // namespace nsb
 #include "nsb_tile.cuh"
 namespace nsb {
@@ -998,6 +1091,7 @@ static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.wbytes = wb;
   K.points = nullptr; K.points_raw = nullptr; K.n_points = 0;
   K.acts_lv = in->stage == NSB_STAGE_COLOR ? 3 : -1;      // the colour decoder is the only one whose weights the mapper optimises (Mapper.py:339-341)
+  memset(&K.smp, 0, sizeof(K.smp));
   for (int l = 0; l < 4; l++) K.d_packed[l] = nullptr;
 }
 
@@ -1155,6 +1249,8 @@ static int set_attrs() {
   if (check_cuda(cudaFuncSetAttribute(render_bwd_wg_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_wg_smem_bytes()), "bwd wg tile smem attr")) return NSB_ERR_CUDA;
   // two CTAs per SM need the full shared-memory carve-out (2 x ~111 KB of the 228 KB)
   if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "fwd tile carveout")) return NSB_ERR_CUDA;
+  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_sampled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem_bytes(false)), "fwd tile (sampled) smem attr")) return NSB_ERR_CUDA;
+  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_sampled_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "fwd tile (sampled) carveout")) return NSB_ERR_CUDA;
   if (check_cuda(cudaFuncSetAttribute(render_bwd_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "bwd tile carveout")) return NSB_ERR_CUDA;
   if (check_cuda(cudaFuncSetAttribute(render_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "fwd smem attr")) return NSB_ERR_CUDA;
   if (check_cuda(cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "bwd smem attr")) return NSB_ERR_CUDA;
@@ -1176,14 +1272,32 @@ extern "C" int nsb_set_option(const char* key, int value) {
   set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
 }
 
-extern "C" int nsb_render_forward(const nsb_render_inputs* in, const nsb_forward_outputs* out, void* stream) {
-  return nsb::render_forward_fused(in, out, nullptr, stream);
+// nsb_sampling -> K.smp; a given sample list sets the samples per ray
+static int apply_sampling(KParams& K, const nsb_sampling* smp) {
+  if (smp == nullptr) return NSB_OK;
+  K.smp = *smp;
+  if (smp->z_vals != nullptr) {
+    if (smp->S < 1) { set_error("nsb_sampling.S = %d with a given z_vals", smp->S); return NSB_ERR_ARG; }
+    K.S = smp->S; K.smp.lindisp = 0; K.smp.t_rand = nullptr;
+  }
+  return NSB_OK;
 }
-int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_outputs* out, const nsb::FusedSeeds* fs, void* stream) {
+
+// Renderer.render_batch_ray, src/utils/Renderer.py:63-198 (nsb_render_forward: the default sampler, Renderer.py:82-170)
+extern "C" int nsb_render_forward(const nsb_render_inputs* in, const nsb_forward_outputs* out, void* stream) {
+  return nsb_render_forward_sampled(in, nullptr, out, stream);
+}
+// lindisp, perturb (Renderer.py:152-166) and the second pass of hierarchical sampling (:181-196)
+extern "C" int nsb_render_forward_sampled(const nsb_render_inputs* in, const nsb_sampling* sampling, const nsb_forward_outputs* out, void* stream) {
+  return nsb::render_forward_fused(in, out, nullptr, stream, sampling);
+}
+int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_outputs* out, const nsb::FusedSeeds* fs, void* stream,
+                              const nsb_sampling* smp) {
   int rc = validate_inputs(in, true); if (rc) return rc;
   if (!out || !out->depth || !out->var || !out->rgb) { set_error("forward outputs missing"); return NSB_ERR_ARG; }
   if (in->n_rays == 0) return NSB_OK;
   KParams K; fill_common(K, in); K.fo = *out; memset(&K.bw, 0, sizeof(K.bw));
+  if ((rc = apply_sampling(K, smp))) return rc;
   if (fs != nullptr) K.fs = *fs;
   const bool sharded = fs != nullptr && fs->px.world > 1;
   const bool tile = use_tile_kernels(K.S, in->n_rays, sharded), group = use_group_kernels(K.S, in->n_rays, sharded);
@@ -1201,7 +1315,9 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
     K.split = w.split; K.ray_cnt = w.ray_cnt;
     K.tile_parts = w.split > 1 ? static_cast<float4*>(w.scratch) : reinterpret_cast<float4*>(out->raw);
     const long long grid_t = tile_count((long long)in->n_rays * K.S) * K.split;
-    if (g_fwd_f16) render_fwd_tile_h16_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
+    // lindisp / perturb / a given sample list: the 3xTF32 instantiation with the full sampler (the default one does not read K.smp)
+    if (K.smp.lindisp || K.smp.t_rand || K.smp.z_vals) render_fwd_tile_sampled_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
+    else if (g_fwd_f16) render_fwd_tile_h16_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
     else render_fwd_tile_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
     return check_cuda(cudaGetLastError(), "render_fwd_tile_kernel launch");
   }
@@ -1259,14 +1375,21 @@ extern "C" size_t nsb_backward_workspace_bytes(void) {
   size_t t = 0; for (int l = 0; l < 4; l++) t += align16((size_t)packed_floats(l) * 4); return t;
 }
 
+// loss.backward() at src/Tracker.py:125 / src/Mapper.py:503 (nsb_render_backward: after the default sampler)
 extern "C" int nsb_render_backward(const nsb_render_inputs* in, const nsb_backward_args* bw, void* stream) {
-  return nsb::render_backward_tail(in, bw, nullptr, stream, false);
+  return nsb_render_backward_sampled(in, nullptr, bw, stream);
 }
-int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_args* bw, const nsb::PeerTail* tail, void* stream, bool after_forward) {
+// backward of nsb_render_forward_sampled (Renderer.py:152-196 put the samples; z comes from bw->z_vals)
+extern "C" int nsb_render_backward_sampled(const nsb_render_inputs* in, const nsb_sampling* sampling, const nsb_backward_args* bw, void* stream) {
+  return nsb::render_backward_tail(in, bw, nullptr, stream, false, sampling);
+}
+int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_args* bw, const nsb::PeerTail* tail, void* stream, bool after_forward,
+                              const nsb_sampling* smp) {
   int rc = validate_inputs(in, true); if (rc) return rc;
   if (!bw || !bw->z_vals || !bw->raw) { set_error("backward needs z_vals and raw from the forward pass"); return NSB_ERR_ARG; }
   if (in->n_rays == 0) return NSB_OK;
   KParams K; fill_common(K, in); K.bw = *bw; memset(&K.fo, 0, sizeof(K.fo));
+  if ((rc = apply_sampling(K, smp))) return rc;
   if (K.S > NSB_MAX_SAMPLES) { set_error("n_samples+n_surface = %d exceeds %d", K.S, NSB_MAX_SAMPLES); return NSB_ERR_UNSUPPORTED; }
   cudaStream_t st = (cudaStream_t)stream;
   bool any_w = false;
@@ -1392,6 +1515,19 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     if (bw->result_dst != nullptr) return nsb_copy_block(bw->result_dst, bw->result_src, bw->result_bytes, stream);
   }
   return NSB_OK;
+}
+
+// Renderer.py:181-185 (sample_pdf, src/common.py:19-63 and the merge of :185)
+extern "C" int nsb_importance_samples(const double* z_vals, const float* raw, int n_rays, int S0, int n_importance, const float* u, int u_per_ray,
+                                      double* z_out, void* stream) {
+  if (n_rays < 0 || S0 < 3 || n_importance < 1) { set_error("importance sampling needs n_rays >= 0, S0 >= 3, n_importance >= 1"); return NSB_ERR_ARG; }
+  if (S0 + n_importance > NSB_MAX_SAMPLES) {
+    set_error("S0 + n_importance = %d exceeds %d", S0 + n_importance, NSB_MAX_SAMPLES); return NSB_ERR_UNSUPPORTED; }
+  if (n_rays == 0) return NSB_OK;
+  if (!z_vals || !raw || !u || !z_out) { set_error("z_vals / raw / u / z_out missing"); return NSB_ERR_ARG; }
+  importance_kernel<<<(n_rays + kImpWarps - 1) / kImpWarps, kImpWarps * 32, 0, (cudaStream_t)stream>>>(z_vals, raw, n_rays, S0, n_importance, u,
+                                                                                                        u_per_ray, z_out);
+  return check_cuda(cudaGetLastError(), "importance_kernel launch");
 }
 
 // resident CTAs per SM of the tile kernels (diagnostic; 2 = the design point)

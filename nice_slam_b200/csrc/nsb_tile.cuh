@@ -1043,7 +1043,7 @@ __device__ __forceinline__ void composite_ray(const KParams& P, int ray, int lan
 // ================================================================================================================================
 // forward kernel
 // ================================================================================================================================
-template <bool H16>
+template <bool H16, bool kSampled = false>
 __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using namespace tl;
@@ -1097,7 +1097,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
     block_setup_rays(P, rays, far, ray_lo, nr, gtmax12);
     __syncthreads();
     NSB_PH(41);
-    block_sample_sort(P, rays, far, nr, gtmax, zu, zs, reinterpret_cast<int*>(zs + (size_t)nr * S));
+    block_sample_sort<kSampled>(P, rays, far, ray_lo, nr, gtmax, zu, zs, reinterpret_cast<int*>(zs + (size_t)nr * S));
     __syncthreads();
     NSB_PH(43);
     {
@@ -1155,6 +1155,8 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false>(P); }
 // forward with FP16 hi|lo operands (option fwd_f16; see mma_rows)
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_h16_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<true>(P); }
+// lindisp / perturb / a given sample list (KParams::smp, nsb_render_forward_sampled)
+__global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_sampled_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false, true>(P); }
 
 // ================================================================================================================================
 // backward kernel (input gradients: rays + grid voxels)

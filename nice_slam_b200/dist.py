@@ -106,6 +106,8 @@ class ShardedTrackingIteration:
 
     def __init__(self, ctx, exchange="auto"):
         """exchange: 'auto' = in-kernel exchanges over NVLink peer memory when available, else NCCL; 'nccl' = NCCL collectives."""
+        from .renderer import require_default_sampling
+        require_default_sampling(ctx.r, "ShardedTrackingIteration")
         self.ctx = ctx                      # steps.IterationContext(kind='track')
         dev = ctx.dev
         self.res = torch.empty(ctx.n, dtype=torch.float64, device=dev)
@@ -253,6 +255,8 @@ class ShardedMappingIteration:
 
     def __init__(self, ctx):
         assert ctx.kind == "map"
+        from .renderer import require_default_sampling
+        require_default_sampling(ctx.r, "ShardedMappingIteration")
         self.ctx = ctx
         self._p = None
 

@@ -9,7 +9,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .renderer import _VP, _stream
+from .renderer import _VP, _stream, require_default_sampling
 
 from ._lib import STAGE_DECODERS
 from .masked import MaskedVoxels, frustum_voxel_mask
@@ -23,6 +23,7 @@ class FusedMappingLoop:
     def __init__(self, renderer, c, decoders, c2w, depth, keys=("grid_middle", "grid_fine", "grid_color"), w_color=0.2, capacity=1024):
         """c: the shared grids dict (updated in place); c2w / depth: pose and sensor depth of the current frame (frustum selection);
         capacity: rays per iteration the buffers are sized for (cfg['mapping']['pixels'])."""
+        require_default_sampling(renderer, "FusedMappingLoop")
         self.r, self.c, self.dec, self.w_color, self.capacity = renderer, c, decoders, w_color, int(capacity)
         self.masked = {k: MaskedVoxels(c[k], frustum_voxel_mask(renderer, c2w, k, c[k], depth)) for k in keys}
         self.adam = FusedMapperAdam()

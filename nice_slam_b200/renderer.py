@@ -108,7 +108,7 @@ class _PackCache:
 class _Call:
     """Non-tensor arguments of one render call."""
     __slots__ = ("stage", "levels", "bound", "cbound", "n_samples", "n_surface", "gt_depth", "packed", "param_names",
-                 "aux", "masked", "grid_data")
+                 "aux", "masked", "grid_data", "lindisp", "t_rand", "z_given")
 
 
 INLINE_MAX_RAYS = 1024          # NSB_INLINE_MAX_RAYS of include/nice_slam_b200.h
@@ -147,8 +147,55 @@ def _linspaces(n_samples, n_surface, device):
     return _LINSPACE[key]
 
 
+def _sampling(call):
+    """nsb_sampling of a call (None: the default sampler, i.e. plain nsb_render_forward / nsb_render_backward)."""
+    if not call.lindisp and call.t_rand is None and call.z_given is None:
+        return None
+    smp = _lib.Sampling()
+    smp.lindisp = 1 if call.lindisp else 0
+    smp.t_rand = _ptr(call.t_rand)
+    if call.z_given is not None:
+        smp.z_vals, smp.S = call.z_given.data_ptr(), call.z_given.shape[1]
+    return C.byref(smp)
+
+
+def _samples_per_ray(call):
+    if call.z_given is not None:
+        return call.z_given.shape[1]
+    has_gt = call.gt_depth is not None and call.stage != "coarse"
+    return call.n_samples + (call.n_surface if has_gt else 0)
+
+
+def _forward_only(call, ro, rd, grids):
+    """The render forward without autograd and without the state a backward would need (saved ReLU masks, layer outputs):
+    the first pass of hierarchical sampling.  Returns z_vals [N,S] f64 and raw [N,S,4]."""
+    L = _lib.lib()
+    dev = ro.device
+    n = ro.shape[0]
+    S = _samples_per_ray(call)
+    depth_max = None
+    if call.gt_depth is not None and n > INLINE_MAX_RAYS:
+        depth_max = torch.empty(2, dtype=torch.float32, device=dev)
+        _lib.check(L.nsb_batch_max_depth(_ptr(call.gt_depth), n, _ptr(depth_max), _stream()), "nsb_batch_max_depth")
+    t_u, t_s = _linspaces(call.n_samples, call.n_surface, dev)
+    inp = _inputs(call, ro, rd, depth_max, t_u, t_s, grids)
+    depth = torch.empty(n, dtype=torch.float64, device=dev)
+    var = torch.empty(n, dtype=torch.float64, device=dev)
+    rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    z_vals = torch.empty(n, S, dtype=torch.float64, device=dev)
+    raw = torch.empty(n, S, 4, dtype=torch.float32, device=dev)
+    nsplit = L.nsb_split_workspace_bytes(n, S)
+    split = torch.zeros(nsplit, dtype=torch.uint8, device=dev) if nsplit else None
+    out = _lib.ForwardOutputs(depth.data_ptr(), var.data_ptr(), rgb.data_ptr(), z_vals.data_ptr(), raw.data_ptr(), None, None,
+                              split.data_ptr() if nsplit else None, nsplit, None)
+    if n > 0:
+        _lib.check(L.nsb_render_forward_sampled(C.byref(inp), _sampling(call), C.byref(out), _stream()), "nsb_render_forward_sampled")
+    return z_vals, raw
+
+
 class _RenderFn(torch.autograd.Function):
-    """forward/backward = nsb_render_forward / nsb_render_backward."""
+    """forward/backward = nsb_render_forward_sampled / nsb_render_backward_sampled (= nsb_render_forward / nsb_render_backward with the
+    default sampler)."""
 
     @staticmethod
     def forward(ctx, call, rays_o, rays_d, *tensors):
@@ -159,8 +206,7 @@ class _RenderFn(torch.autograd.Function):
         ro = rays_o.detach().contiguous().float()
         rd = rays_d.detach().contiguous().float()
         n = ro.shape[0]
-        has_gt = call.gt_depth is not None and call.stage != "coarse"
-        S = call.n_samples + (call.n_surface if has_gt else 0)
+        S = _samples_per_ray(call)
         depth_max = None
         if call.gt_depth is not None and n > INLINE_MAX_RAYS:             # smaller batches: the render kernel reduces gt_depth itself
             depth_max = torch.empty(2, dtype=torch.float32, device=dev)
@@ -192,7 +238,7 @@ class _RenderFn(torch.autograd.Function):
             corner = torch.empty(n, S, 3, dtype=torch.int32, device=dev)
             out.corner_idx = corner.data_ptr()
         if n > 0:                                                         # (an empty batch has no storage to point at)
-            _lib.check(L.nsb_render_forward(C.byref(inp), C.byref(out), _stream()), "nsb_render_forward")
+            _lib.check(L.nsb_render_forward_sampled(C.byref(inp), _sampling(call), C.byref(out), _stream()), "nsb_render_forward_sampled")
         if call.aux is not None:
             call.aux.update(z_vals=z_vals, raw=raw, corner_idx=corner, masks=masks)
         ctx.call = call
@@ -268,13 +314,22 @@ class _RenderFn(torch.autograd.Function):
             ws = torch.empty(L.nsb_backward_workspace_bytes(), dtype=torch.uint8, device=dev)
             bw.workspace = ws.data_ptr()
         if n > 0:
-            _lib.check(L.nsb_render_backward(C.byref(inp), C.byref(bw), _stream()), "nsb_render_backward")
+            _lib.check(L.nsb_render_backward_sampled(C.byref(inp), _sampling(call), C.byref(bw), _stream()), "nsb_render_backward_sampled")
         elif d_o is not None:
             d_o.zero_(); d_d.zero_()
         for j, dg in compact.items():
             mv = call.masked[j]
             d_grids[j] = mv.to_reference(dg[: mv.count]) if mv.count > 0 else torch.zeros(0, dtype=torch.float32, device=dev)
         return (None, d_o if needs[1] else None, d_d if needs[2] else None, *d_grids, *d_params)
+
+
+def require_default_sampling(renderer, what):
+    """The fused iteration and mapping-loop classes build their own sampling inputs (linspaces, one pass): they refuse a renderer configured
+    for lindisp, perturb or importance sampling instead of silently rendering without them."""
+    lindisp, perturb, n_imp = getattr(renderer, "lindisp", False), getattr(renderer, "perturb", 0), getattr(renderer, "N_importance", 0)
+    if lindisp or perturb > 0 or n_imp > 0:
+        raise RuntimeError("%s supports lindisp=False, perturb=0, N_importance=0 only (got lindisp=%r, perturb=%r, N_importance=%r); "
+                           "render through FusedRenderer.render_batch_ray" % (what, lindisp, perturb, n_imp))
 
 
 class FusedRenderer(object):
@@ -292,8 +347,6 @@ class FusedRenderer(object):
         self.coarse_bound_enlarge = cfg["model"]["coarse_bound_enlarge"]
         if not self.nice or not self.occupancy:
             raise RuntimeError("FusedRenderer implements the NICE (occupancy) path only; iMAP* stays on the reference Renderer")
-        if self.lindisp or self.perturb > 0 or self.N_importance > 0:
-            raise RuntimeError("FusedRenderer supports lindisp=False, perturb=0, N_importance=0 (configs/nice_slam.yaml:105-110)")
         if convert_grids and getattr(slam, "shared_c", None) is not None:
             to_channels_last(slam.shared_c)        # layout conversion point, before Mapper/Tracker capture the dict
         self._cache = _PackCache()
@@ -337,6 +390,7 @@ class FusedRenderer(object):
         call.param_names = {lvl: [nm for nm, _, _ in _lib.flat_layout(LEVELS.index(lvl))] for lvl in call.levels}
         call.aux = aux
         call.masked, call.grid_data = [None] * len(call.levels), [None] * len(call.levels)
+        call.lindisp, call.t_rand, call.z_given = bool(self.lindisp), None, None
         grids = [c["grid_" + lvl] for lvl in call.levels]
         plist = [params[lvl][nm] for lvl in call.levels for nm in call.param_names[lvl]]
         return call, grids, plist
@@ -344,10 +398,33 @@ class FusedRenderer(object):
     # ------------------------------------------------------------------ reference API
     def render_batch_ray(self, c, decoders, rays_d, rays_o, device, stage, gt_depth=None, aux=None):
         """Render depth, uncertainty and colour of a batch of rays (Renderer.render_batch_ray, Renderer.py:63-198).
-        `aux` (optional dict) receives z_vals / raw / corner_idx / masks (the saved ReLU words) for the parity tests."""
+        `aux` (optional dict) receives z_vals / raw / corner_idx / masks (the saved ReLU words) for the parity tests; with importance
+        sampling z_vals / raw are those of the second pass, and z_vals0 / raw0 those of the first.
+        perturb > 0 and N_importance > 0 draw their uniforms from the default CPU generator exactly as the reference does
+        (torch.rand, Renderer.py:165 and common.py:37), so the caller's random stream advances the same way."""
         _require_cuda(rays_o, "rays_o")
         _require_cuda(rays_d, "rays_d")
         call, grids, plist = self._call(c, decoders, stage, gt_depth, rays_o.device, aux)
+        n = rays_o.shape[0]
+        if self.perturb > 0:
+            call.t_rand = torch.rand([n, self.N_samples]).to(rays_o.device)                         # Renderer.py:165
+        if self.N_importance > 0:
+            # Renderer.py:181-196: pass 1 only places the samples (no autograd, its outputs are discarded); pass 2 renders the merged list
+            ro = rays_o.detach().contiguous().float()
+            rd = rays_d.detach().contiguous().float()
+            z0, raw0 = _forward_only(call, ro, rd, [g.detach() for g in grids])
+            if self.perturb == 0:
+                u, per_ray = torch.linspace(0., 1., steps=self.N_importance), 0                    # sample_pdf(det=True), common.py:34-36
+            else:
+                u, per_ray = torch.rand([n, self.N_importance]), 1                                   # common.py:37-38
+            u = u.to(rays_o.device).contiguous()
+            S0 = z0.shape[1]
+            z = torch.empty(n, S0 + self.N_importance, dtype=torch.float64, device=rays_o.device)
+            _lib.check(_lib.lib().nsb_importance_samples(_ptr(z0), _ptr(raw0), n, S0, self.N_importance, _ptr(u), per_ray, _ptr(z), _stream()),
+                       "nsb_importance_samples")
+            call.lindisp, call.t_rand, call.z_given = False, None, z
+            if aux is not None:
+                aux.update(z_vals0=z0, raw0=raw0)
         if self.detect_masked_grids and torch.is_grad_enabled():
             for j, g in enumerate(grids):
                 sel = self._masked_leaf(g)

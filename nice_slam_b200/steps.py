@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import LEVELS, STAGE_DECODERS
-from .renderer import _VP, _inputs, _linspaces, _stream, _Call, _require_cuda
+from .renderer import _VP, _inputs, _linspaces, _stream, _Call, _require_cuda, require_default_sampling
 
 KERNEL_LAUNCHES_PER_ITERATION = 2       # render_fwd + render_bwd for batches <= 1024 rays: the forward reduces the batch depth maxima itself and
                                         # its last CTA computes the loss seeds, the backward's last CTA produces d c2w; larger batches add
@@ -41,6 +41,7 @@ class IterationContext:
                  masked=None, n_frames=0, host_staging=True):
         """masked: {grid key: masked.MaskedVoxels} -- those grids get COMPACT [n_selected,32] gradients (Mapper.py:317-333) instead of
         dense ones; n_frames: keyframes of the bundle-adjustment window whose d c2w is wanted (pose_grad_frames)."""
+        require_default_sampling(renderer, "IterationContext")
         L = _lib.lib()
         self.r, self.n, self.stage, self.kind = renderer, int(n_rays), stage, kind
         self.n_last = self.n                  # rays of the last run() (<= capacity n)
