@@ -111,6 +111,9 @@ __device__ __forceinline__ void wg_commit_wait() {
 }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the N most recently committed MMA groups of this warpgroup have completed
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving reads of a register accumulator above the wgmma.wait that completes it
 __device__ __forceinline__ void fence_acc(float (&d)[16]) {
 #pragma unroll
@@ -131,6 +134,23 @@ __device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t da, uint6
                "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
                : NSB_WG_D16 : "l"(da), "l"(db));
+}
+// [d0 | d1][64 x 64] += A * B[64 x K]^T: one instruction for two adjacent 32-column accumulators (A is read once for both).  The m64n64
+// fragment is the two m64n32 fragments one after the other: its elements 0..15 are columns 0..31, elements 16..31 columns 32..63.
+#define NSB_WG_D32 "+f"(d0[0]), "+f"(d0[1]), "+f"(d0[2]), "+f"(d0[3]), "+f"(d0[4]), "+f"(d0[5]), "+f"(d0[6]), "+f"(d0[7]), \
+                   "+f"(d0[8]), "+f"(d0[9]), "+f"(d0[10]), "+f"(d0[11]), "+f"(d0[12]), "+f"(d0[13]), "+f"(d0[14]), "+f"(d0[15]), \
+                   "+f"(d1[0]), "+f"(d1[1]), "+f"(d1[2]), "+f"(d1[3]), "+f"(d1[4]), "+f"(d1[5]), "+f"(d1[6]), "+f"(d1[7]), \
+                   "+f"(d1[8]), "+f"(d1[9]), "+f"(d1[10]), "+f"(d1[11]), "+f"(d1[12]), "+f"(d1[13]), "+f"(d1[14]), "+f"(d1[15])
+#define NSB_WG_R32 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d0)[16], float (&d1)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " NSB_WG_R32 ", %32, %33, p, 1, 1;\n\t}"
+               : NSB_WG_D32 : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_f16_n64(float (&d0)[16], float (&d1)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " NSB_WG_R32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : NSB_WG_D32 : "l"(da), "l"(db));
 }
 // Fragment of m64n32: element e of thread (warp w of the warpgroup, lane l) is row 16 w + l / 4 + 8 ((e >> 1) & 1), column 8 (e >> 2) + 2 (l & 3) + (e & 1).
 __device__ __forceinline__ void frag_rc(int e, int& r, int& c) {

@@ -228,29 +228,53 @@ __device__ __forceinline__ void put16_h(float* tile, int r, int cg, const float 
 // wgmma.fence and commit_group a straight run of wgmma with compile-time unit and k-step counts, reached by every thread of the warpgroup;
 // accumulators initialised just before the fence (a constant zero kept in the open, as in the coarse layer 0, is materialised by ptxas
 // inside the group, hence zero16_opaque); producer work and mbarrier waits before them; every group waited for on every path that leads
-// to a read of its accumulators.
-template <bool H16, int ksteps>
-__device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0, const float* b, int N, int KB, int c) {
+// to a read of its accumulators.  A group may stay in flight across other code (the layer-0 chain) if that code has no branch or predicated
+// instruction ptxas may take as divergent (C7518) and every wait follows a whole group in the code.
+struct RowsDesc { uint64_t ah, al, bh, bl; };      // hi / lo descriptors of this warpgroup's A rows and of B from row 32 c
+template <bool H16>
+__device__ __forceinline__ RowsDesc rows_desc(const float* a, int ka0, const float* b, int N, int KB, int c) {
   const uint32_t g = (threadIdx.x >> 7) & 1u;
   const int esz = H16 ? 2 : 4, kcm = H16 ? 8 : 4;               // bytes per element, elements per 16-byte core-matrix row
   const uint32_t sbo_a = (32u / kcm) * 128u, sbo_b = (uint32_t)(KB / kcm) * 128u;
-  uint64_t ah = tc::make_desc(a + (ka0 / kcm) * 32, 128u, sbo_a), bh = tc::make_desc(b, 128u, sbo_b);
-  ah += (uint64_t)((8u * sbo_a * g) >> 4);
-  bh += (uint64_t)((4u * sbo_b * (uint32_t)c) >> 4);
-  const uint64_t al = ah + (uint64_t)((TM * 32 * esz) >> 4), bl = bh + (uint64_t)((N * KB * esz) >> 4);
+  RowsDesc r;
+  r.ah = tc::make_desc(a + (ka0 / kcm) * 32, 128u, sbo_a) + (uint64_t)((8u * sbo_a * g) >> 4);
+  r.bh = tc::make_desc(b, 128u, sbo_b) + (uint64_t)((4u * sbo_b * (uint32_t)c) >> 4);
+  r.al = r.ah + (uint64_t)((TM * 32 * esz) >> 4); r.bl = r.bh + (uint64_t)((N * KB * esz) >> 4);
+  return r;
+}
+template <bool H16, int ksteps>
+__device__ __forceinline__ void mma_rows(float (&d)[16], const float* a, int ka0, const float* b, int N, int KB, int c) {
+  const RowsDesc r = rows_desc<H16>(a, ka0, b, N, KB, c);
 #pragma unroll
   for (int ks = 0; ks < ksteps; ks++) {
     const uint64_t o = 16u * (uint64_t)ks;
-    if (H16) { tc::wgmma_f16_n32(d, al + o, bh + o); tc::wgmma_f16_n32(d, ah + o, bl + o); tc::wgmma_f16_n32(d, ah + o, bh + o); }
-    else { tc::wgmma_tf32_n32(d, al + o, bh + o); tc::wgmma_tf32_n32(d, ah + o, bl + o); tc::wgmma_tf32_n32(d, ah + o, bh + o); }
+    if (H16) { tc::wgmma_f16_n32(d, r.al + o, r.bh + o); tc::wgmma_f16_n32(d, r.ah + o, r.bl + o); tc::wgmma_f16_n32(d, r.ah + o, r.bh + o); }
+    else { tc::wgmma_tf32_n32(d, r.al + o, r.bh + o); tc::wgmma_tf32_n32(d, r.ah + o, r.bl + o); tc::wgmma_tf32_n32(d, r.ah + o, r.bh + o); }
   }
 }
-// this warpgroup's MMAs on the next `count` units have completed: one arrival per warpgroup on each unit's `empty` barrier (and on `done`)
-__device__ __forceinline__ void release_units(Issuer& I, const TileSmem& t, uint32_t count, uint64_t* done = nullptr) {
+// the same for B rows [32 c, 32 c + 64) into [d0 | d1] with m64n64 instructions: every element sees the products of mma_rows on d0 (c) and
+// d1 (c + 1) in the same order, with half the instructions and one read of the A slice instead of two
+template <bool H16, int ksteps>
+__device__ __forceinline__ void mma_rows64(float (&d0)[16], float (&d1)[16], const float* a, int ka0, const float* b, int N, int KB, int c) {
+  const RowsDesc r = rows_desc<H16>(a, ka0, b, N, KB, c);
+#pragma unroll
+  for (int ks = 0; ks < ksteps; ks++) {
+    const uint64_t o = 16u * (uint64_t)ks;
+    if (H16) { tc::wgmma_f16_n64(d0, d1, r.al + o, r.bh + o); tc::wgmma_f16_n64(d0, d1, r.ah + o, r.bl + o); tc::wgmma_f16_n64(d0, d1, r.ah + o, r.bh + o); }
+    else { tc::wgmma_tf32_n64(d0, d1, r.al + o, r.bh + o); tc::wgmma_tf32_n64(d0, d1, r.ah + o, r.bl + o); tc::wgmma_tf32_n64(d0, d1, r.ah + o, r.bh + o); }
+  }
+}
+// this warpgroup's MMAs on units [first, first + count) of the consumption order have completed: one arrival per warpgroup on each unit's
+// `empty` barrier (and on `done`)
+__device__ __forceinline__ void arrive_units(const TileSmem& t, uint32_t first, uint32_t count, uint64_t* done = nullptr) {
   if ((threadIdx.x & 127) == 0) {
-    for (uint32_t k = 0; k < count; k++) mbar_arrive(t.bars + B_EMPTY + ((I.issued + k) & (kSlots - 1)));
+    for (uint32_t k = 0; k < count; k++) mbar_arrive(t.bars + B_EMPTY + ((first + k) & (kSlots - 1)));
     if (done != nullptr) mbar_arrive(done);
   }
+}
+// ... on the next `count` units
+__device__ __forceinline__ void release_units(Issuer& I, const TileSmem& t, uint32_t count, uint64_t* done = nullptr) {
+  arrive_units(t, I.issued, count, done);
   I.issued += count;
 }
 __device__ __forceinline__ void wg_bar_sync() {                 // named barrier of this warpgroup's 128 threads (ids 1, 2; 0 is __syncthreads)
@@ -383,43 +407,60 @@ __device__ __forceinline__ void st_frag(float4* p, const float (&d)[16]) {
 #pragma unroll
   for (int k = 0; k < 4; k++) p[k] = make_float4(d[4 * k], d[4 * k + 1], d[4 * k + 2], d[4 * k + 3]);
 }
-template <bool H16 = false>
-__device__ __forceinline__ void issue_fc(Issuer& I, const TileSmem& t, int half) {       // C tile `half` -> D2 (+)= C * Wc^T
+// C tile `half` -> D2 (+)= C * Wc^T in three MMA groups: chunks (0, 1) and (2, 3) as one 64-column group each into [d1 | d3] (dead until
+// layer 0), chunk 4 as a 32-column group into d1; each group is waited for and stored before the next one reuses the registers.  The half's
+// units and operand buffer are released after the last group.  kAccumulate: C half 1 adds onto the chunks of half 0 (a template argument:
+// each group's accumulators are set up by straight-line code).  Per element the products come in the order of one m64n32 group per chunk.
+template <bool H16, bool kAccumulate>
+__device__ __forceinline__ void issue_fc(Issuer& I, const TileSmem& t, float (&d1)[16], float (&d3)[16]) {
   constexpr int nu = H16 ? 2 : 4;                                // units of one C half: [160 x 16] FP16 / [160 x 8] tf32 (all in the ring at once)
   const int b = I.g & 1;
   issuer_wait_operands(I, t, b, (I.g >> 1) & 1u);
+  NSB_PH(5);
 #pragma unroll 1
   for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
-#pragma unroll 1
-  for (int c = 0; c < 5; c++) {                                  // chunk c = fc_c of layer c
-    float4* p = d2_frag(c);
-    float d[16];
-    if (half == 0) zero16(d); else ld_frag(p, d);
+  NSB_PH(11);
+#pragma unroll
+  for (int c = 0; c < 5; c += 2) {                               // chunk c = fc_c of layer c
+    const bool pair = c < 4;
+    if (kAccumulate) { ld_frag(d2_frag(c), d1); if (pair) ld_frag(d2_frag(c + 1), d3); }
+    else { zero16_opaque(d1); if (pair) zero16_opaque(d3); }
     tc::wg_fence();
 #pragma unroll
-    for (int u = 0; u < nu; u++) mma_rows<H16, 1>(d, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c);
-    tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d);
-    st_frag(p, d);
+    for (int u = 0; u < nu; u++) {
+      if (pair) mma_rows64<H16, 1>(d1, d3, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c);
+      else mma_rows<H16, 1>(d1, t.a[b], H16 ? 16 * u : 8 * u, issued_unit(I, t, u), 160, H16 ? 16 : 8, c);
+    }
+    tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d1);
+    st_frag(d2_frag(c), d1);
+    if (pair) { tc::fence_acc(d3); st_frag(d2_frag(c + 1), d3); }
   }
   release_units(I, t, nu, t.bars + B_DONE + b);
   I.g++;
 }
+// [D1 | D3] += E_blk * [W0_blk; W3E_blk]^T  (coarse: E = C).  The blocks of layer 0 are one chain of groups on the same accumulators, committed
+// without a wait: the next block's embedding is computed while this block's MMAs run.  The caller retires the groups (wait_group) and then
+// releases their units and operand buffers (release_l0).
 template <bool H16 = false>
-__device__ __forceinline__ void issue_l0(Issuer& I, const TileSmem& t, float (&d1)[16], float (&d3)[16]) {   // [D1 | D3] += E_blk * [W0_blk; W3E_blk]^T  (coarse: E = C)
+__device__ __forceinline__ void issue_l0(Issuer& I, const TileSmem& t, float (&d1)[16], float (&d3)[16]) {
   constexpr int nu = H16 ? 1 : 2;                                // one [64 x 32] FP16 unit / two [64 x 16] tf32 units
   const int b = I.g & 1;
   issuer_wait_operands(I, t, b, (I.g >> 1) & 1u);
+  NSB_PH(10);
 #pragma unroll 1
-  for (int u = 0; u < nu; u++) issuer_unit(I, t, u);
+  for (int u = 0; u < nu; u++) issuer_unit(I, t, u);             // (the ring holds this block's and the previous block's units)
   tc::wg_fence();
 #pragma unroll
-  for (int u = 0; u < nu; u++) {
-    mma_rows<H16, 2>(d1, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 0);
-    mma_rows<H16, 2>(d3, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 1);
-  }
-  tc::wg_commit(); tc::wg_wait0(); tc::fence_acc(d1); tc::fence_acc(d3);
-  release_units(I, t, nu, t.bars + B_DONE + b);
+  for (int u = 0; u < nu; u++) mma_rows64<H16, 2>(d1, d3, t.a[b], 16 * u, issued_unit(I, t, u), 64, H16 ? 32 : 16, 0);
+  tc::wg_commit();
+  I.issued += nu;
   I.g++;
+}
+// layer-0 groups I.g - back .. I.g - back + count - 1 have completed in this warpgroup: release their units and operand buffers
+template <bool H16 = false>
+__device__ __forceinline__ void release_l0(const Issuer& I, const TileSmem& t, uint32_t back, uint32_t count) {
+  constexpr uint32_t nu = H16 ? 1 : 2;
+  for (uint32_t j = back; j > back - count; j--) arrive_units(t, I.issued - j * nu, nu, t.bars + B_DONE + ((I.g - j) & 1u));
 }
 // layer i (1..4) of this warpgroup's rows from its rows of the H tile of layer i-1 into d1 (layer 3 accumulates onto D3); committed, not waited for
 template <bool H16 = false>
@@ -445,8 +486,7 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
   const bool xyz = lv != 0;
   const int cd = op_cd(lv), no = lv == 3 ? 4 : 1;
   const float* hdr = t.hdr + hb * kHdrFloats;
-  float d1[16], d3[16];
-  zero16(d1); zero16(d3);                                        // (here, not at the first block: the compiler then sees them dead until layer 0)
+  float d1[16], d3[16];                                          // (the fc_c chunks pass through them before layer 0)
   if (xyz) {
     for (int half = 0; half < cd / 32; half++) {
       if (n >= 2) wait_group(t, n - 2);
@@ -454,11 +494,13 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
       gather_tile<H16>(P.in.grid[half == 0 ? lv : 1], t.a[n & 1], G.xn, warp, lane);
       NSB_PH(1);
       publish(t, n & 1); n++;
-      issue_fc<H16>(I, t, half);
+      if (half == 0) issue_fc<H16, false>(I, t, d1, d3); else issue_fc<H16, true>(I, t, d1, d3);
       NSB_PH(2);
     }
     mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
-    for (int blk = 0; blk < 3; blk++) {
+    zero16_opaque(d1); zero16_opaque(d3);                        // (straight-line zeros would be materialised inside the MMA group)
+#pragma unroll
+    for (int blk = 0; blk < 3; blk++) {                          // (unrolled: every wait below follows a whole MMA group in the code)
       if (n >= 2) wait_group(t, n - 2);
       if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);
       NSB_PH(6);
@@ -466,19 +508,23 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
       NSB_PH(3);
       publish(t, n & 1); n++;
       issue_l0<H16>(I, t, d1, d3);
+      // the ring holds two blocks' units: block 0 is retired here to make room for block 2's
+      if (blk == 1) { tc::wg_wait<1>(); release_l0<H16>(I, t, 2, 1); }
       NSB_PH(4);
     }
   } else {
     if (n >= 2) wait_group(t, n - 2);
     gather_tile<H16>(P.in.grid[0], t.a[n & 1], G.xnc, warp, lane);
     publish(t, n & 1); n++;
-    zero16_opaque(d1); zero16_opaque(d3);                        // (straight-line zeros would be materialised inside the MMA group)
+    zero16_opaque(d1); zero16_opaque(d3);
     issue_l0<H16>(I, t, d1, d3);
     mbar_wait_b(t.bars + B_HDR + hb, hdr_parity);
   }
+  tc::wg_wait0(); tc::fence_acc(d1); tc::fence_acc(d3);          // layer 0 has completed
+  release_l0<H16>(I, t, xyz ? 2 : 1, xyz ? 2 : 1);
   st_frag(d2_frag(5), d3);                                       // D3 waits for layer 3 in the slot (fewer live registers in layers 1, 2)
-  // Hidden layers.  H tiles go to buffer n & 1: its last group (n - 2) completed in both warpgroups before group n - 1 was published, and each
-  // warpgroup writes and reads only its own rows of it.
+  // Hidden layers.  H tiles go to buffer n & 1: every group of this warpgroup has completed (the wait above), and each warpgroup writes and reads
+  // only its own rows of it.
   float* hbuf = t.a[n & 1];
   const int wg = threadIdx.x >> 7, q = lane & 3;
   const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);        // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8

@@ -15,8 +15,10 @@ from nice_slam_b200 import _lib  # noqa: E402
 from nice_slam_b200.steps import IterationContext  # noqa: E402
 
 TILE_NAMES = {40: "fwd: launch -> depth max done", 41: "fwd: ray table (bbox far, near)", 43: "fwd: sample z + rank sort", 44: "fwd: point geometry + syncs",
-              1: "fwd: gather (per grid)", 2: "fwd: publish + issue fc_c", 6: "fwd: wait free buffer (E block)", 3: "fwd: embed block compute", 4: "fwd: publish + issue layer-0 block",
-              7: "fwd: wait MMAs of the layer", 8: "fwd: layer epilogue (relu, masks, H write)", 9: "fwd: publish + issue hidden layer", 12: "fwd: output layer + syncs",
+              1: "fwd: gather (per grid)", 5: "fwd: publish + wait all warps' gather", 11: "fwd: wait fc_c weight units (TMA)",
+              2: "fwd: issue + complete fc_c MMAs", 6: "fwd: wait free buffer (E block)",
+              3: "fwd: embed block compute", 10: "fwd: publish + wait all warps' E block", 4: "fwd: issue layer-0 block (+ retire block 0)",
+              7: "fwd: wait MMAs of the layer (layer 0: its whole chain)", 8: "fwd: layer epilogue (relu, masks, H write)", 9: "fwd: publish + issue hidden layer", 12: "fwd: output layer + syncs",
               14: "fwd: dealloc + sync", 15: "fwd: parts store + ray completion", 16: "fwd: compositing of completed rays",
               20: "bwd: launch -> ray prologue (weights, dL/docc)", 21: "bwd: point geometry + sync", 22: "bwd: layer epilogue (G/DU write)", 23: "bwd: issue + wait layer MMAs", 24: "bwd: weight-gradient groups (WG)",
               27: "bwd: dc rows + cos chain", 29: "bwd: scatter + dp", 30: "bwd: per-ray partial sums", 31: "bwd: ray completion", 32: "bwd: final ray reduce"}
