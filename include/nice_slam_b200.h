@@ -131,9 +131,11 @@ typedef struct {
   int32_t* corner_idx;           /* optional [N,S,3]: (ix0,iy0,iz0) of the stage's finest occupancy grid */
   uint32_t* masks;               /* optional [N,S,15]: ReLU sign bits of the 5 layers of up to 3 decoders (stage order); when the
                                     backward pass receives them it does not recompute the forward (tensor-core backend only) */
-  void* split_workspace;         /* optional device scratch of nsb_split_workspace_bytes(N, S) bytes, ZEROED ONCE by the caller (the library
-                                    leaves it clean): lets small batches (N <= 256 rays, several decoders) run one CTA per decoder
-                                    and ray group instead of one CTA per ray group; NULL = never split */
+  void* split_workspace;         /* device scratch of nsb_split_workspace_bytes(N, S) bytes, 16-byte aligned, ZEROED ONCE by the caller (the
+                                    library leaves it clean): ray-completion counters and per-item scratch of the tile kernels, which
+                                    refuse a call without it (NSB_ERR_ARG); the round-1 ray-group kernels use it to run small batches
+                                    (N <= 256 rays, several decoders) one CTA per decoder and ray group.  Only the FP32-FMA back-end
+                                    and the round-1 kernels accept NULL. */
   size_t split_workspace_bytes;
   float* acts;                   /* optional [N,S,5,32] float32: outputs of the five hidden layers of the decoder whose WEIGHT gradients the
                                     backward will be asked for (the colour decoder in stage color, src/Mapper.py:339-341).  When the forward
@@ -141,7 +143,8 @@ typedef struct {
                                     the points of a tile) instead of the FP32-FMA pass that recomputes the forward.  NULL = not kept. */
 } nsb_forward_outputs;
 
-/* 0 when the batch is too large to profit from decoder-parallel CTAs. */
+/* Bytes of nsb_forward_outputs.split_workspace for n_rays rays of n_samples_total samples; non-zero for every n_rays >= 1 (0 for
+   n_rays < 1 or n_samples_total < 1).  n_samples_total >= NSB_MAX_SAMPLES sizes a buffer that serves any S. */
 size_t nsb_split_workspace_bytes(int n_rays, int n_samples_total);
 
 /* Forward: sample -> gather -> decode -> composite  (Renderer.render_batch_ray, src/utils/Renderer.py:63-198) */

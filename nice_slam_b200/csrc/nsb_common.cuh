@@ -22,6 +22,8 @@ constexpr int kRowF = 16;           // floats per activation row (one value per 
 constexpr int kMaxPtsPerBlock = 384;
 constexpr int kMaxRaysPerBlock = 24;
 
+__host__ __device__ inline size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
+
 // ---------------------------------------------------------------------------------------------
 // Per-level decoder shape + packed layout (offsets in floats, every block 16-byte aligned)
 // ---------------------------------------------------------------------------------------------

@@ -6,18 +6,16 @@
 
 using namespace nsb;
 
-static size_t a16(size_t x) { return (x + 15) & ~size_t(15); }
-
 // workspace = [fused-seeds counter (16 B) | tracking-seeds scratch | packed weight-gradient images | tile-kernel workspace = the rest].
 // Only the first 16 bytes and the END of the buffer (ray completion counters, nsb_render.cu) hold state that must stay zero between calls,
 // so one buffer sized for a capacity serves batches of varying size.
 static size_t split_bytes(int n_rays) { return nsb_split_workspace_bytes(n_rays, NSB_MAX_SAMPLES); }
 extern "C" size_t nsb_iteration_workspace_bytes(int n_rays) {
-  return 16 + a16(nsb_tracking_seeds_workspace(n_rays)) + a16(nsb_backward_workspace_bytes()) + a16(split_bytes(n_rays));
+  return 16 + align16(nsb_tracking_seeds_workspace(n_rays)) + align16(nsb_backward_workspace_bytes()) + align16(split_bytes(n_rays));
 }
-static int* seeds_counter(const nsb_iteration_buffers* b, int) { return reinterpret_cast<int*>(b->workspace); }
+static int* seeds_counter(const nsb_iteration_buffers* b) { return reinterpret_cast<int*>(b->workspace); }
 static void* seeds_scratch(const nsb_iteration_buffers* b) { return reinterpret_cast<char*>(b->workspace) + 16; }
-static size_t split_offset(int n_rays) { return 16 + a16(nsb_tracking_seeds_workspace(n_rays)) + a16(nsb_backward_workspace_bytes()); }
+static size_t split_offset(int n_rays) { return 16 + align16(nsb_tracking_seeds_workspace(n_rays)) + align16(nsb_backward_workspace_bytes()); }
 static void* split_ptr(const nsb_iteration_buffers* b, int n_rays) { return reinterpret_cast<char*>(b->workspace) + split_offset(n_rays); }
 static size_t split_room(const nsb_iteration_buffers* b, int n_rays) { return b->workspace_bytes - split_offset(n_rays); }
 
@@ -32,25 +30,34 @@ static int check_buffers(const nsb_render_inputs* in, const nsb_iteration_buffer
 static int forward_part(const nsb_render_inputs* in, const nsb_iteration_buffers* b, nsb_render_inputs* in2, const FusedSeeds* fs, void* stream,
                         bool keep_depth_max = false) {
   *in2 = *in;
-  int rc;
-  if (keep_depth_max && in->depth_max != nullptr) {                // the caller supplies the batch depth maxima (sharded batch: maxima of the FULL batch)
-    nsb_forward_outputs fo = {b->depth, b->var, b->rgb, b->z_vals, b->raw, nullptr, b->masks, split_ptr(b, in->n_rays), split_room(b, in->n_rays), b->acts};
-    return render_forward_fused(in2, &fo, fs, stream);
-  }
-  in2->depth_max = nullptr;
-  if (in->gt_depth && in->gt_depth_batch == nullptr && in->n_rays > NSB_INLINE_MAX_RAYS) {          // small batches: the render kernel reduces gt_depth itself
-    if ((rc = nsb_batch_max_depth(in->gt_depth, in->n_rays, b->depth_max, stream))) return rc;
-    in2->depth_max = b->depth_max;
+  if (!(keep_depth_max && in->depth_max != nullptr)) {             // else the caller supplies the batch depth maxima (sharded batch: maxima of the FULL batch)
+    in2->depth_max = nullptr;
+    if (in->gt_depth && in->gt_depth_batch == nullptr && in->n_rays > NSB_INLINE_MAX_RAYS) {        // small batches: the render kernel reduces gt_depth itself
+      const int rc = nsb_batch_max_depth(in->gt_depth, in->n_rays, b->depth_max, stream); if (rc) return rc;
+      in2->depth_max = b->depth_max;
+    }
   }
   nsb_forward_outputs fo = {b->depth, b->var, b->rgb, b->z_vals, b->raw, nullptr, b->masks, split_ptr(b, in->n_rays), split_room(b, in->n_rays), b->acts};
   return render_forward_fused(in2, &fo, fs, stream);
+}
+
+// loss seeds computed by the forward's last CTA into the iteration buffers: kind 1 = tracking (with the residual scratch of the median),
+// 2 = mapping; px: the exchange of a ray-sharded batch, or NULL
+static FusedSeeds fused_seeds(const nsb_iteration_buffers* b, int kind, const void* gt_rgb, const float* gt_depth_loss, double w_color,
+                              int handle_dynamic, int use_color, const PeerX* px) {
+  FusedSeeds fs; memset(&fs, 0, sizeof(fs));
+  fs.kind = kind; fs.gt_rgb = gt_rgb; fs.gt_depth_loss = gt_depth_loss; fs.w_color = w_color; fs.handle_dynamic = handle_dynamic; fs.use_color = use_color;
+  fs.g_depth = b->g_depth; fs.g_rgb = b->g_rgb; fs.loss = b->loss; fs.counter = seeds_counter(b);
+  if (kind == 1) fs.res = static_cast<double*>(seeds_scratch(b));
+  if (px != nullptr) fs.px = *px;
+  return fs;
 }
 
 static int backward_part(const nsb_render_inputs* in2, const nsb_iteration_buffers* b, const nsb_backward_args* g, void* stream, const PeerTail* tail = nullptr,
                          bool after_forward = false) {
   nsb_backward_args bw = *g;
   bw.z_vals = b->z_vals; bw.raw = b->raw; bw.g_depth = b->g_depth; bw.g_var = nullptr; bw.g_rgb = b->g_rgb; bw.masks = b->masks; bw.acts = b->acts;
-  bw.workspace = reinterpret_cast<char*>(b->workspace) + 16 + a16(nsb_tracking_seeds_workspace(in2->n_rays));
+  bw.workspace = reinterpret_cast<char*>(b->workspace) + 16 + align16(nsb_tracking_seeds_workspace(in2->n_rays));
   bw.split_workspace = split_ptr(b, in2->n_rays); bw.split_workspace_bytes = split_room(b, in2->n_rays);
   if (b->event_bwd_begin) cudaEventRecord((cudaEvent_t)b->event_bwd_begin, (cudaStream_t)stream);
   const int rc = render_backward_tail(in2, &bw, tail, stream, after_forward && !b->event_bwd_begin);
@@ -65,13 +72,8 @@ extern "C" int nsb_tracking_iteration(const nsb_render_inputs* in, const nsb_ite
   nsb_render_inputs in2;
   // small batches: the last CTA of the forward launch computes the loss seeds itself (no separate single-CTA launch)
   const bool fuse = in->n_rays > 0 && in->n_rays <= 512;          // (the median by direct rank counting, nsb_seeds.cuh)
-  FusedSeeds fs; memset(&fs, 0, sizeof(fs));
-  if (fuse) {
-    fs.kind = 1; fs.gt_rgb = gt_rgb; fs.w_color = w_color; fs.handle_dynamic = handle_dynamic; fs.use_color = use_color;
-    fs.g_depth = buf->g_depth; fs.g_rgb = buf->g_rgb; fs.loss = buf->loss; fs.res = static_cast<double*>(seeds_scratch(buf));
-    fs.counter = seeds_counter(buf, in->n_rays);
-    if (use_color && !gt_rgb) { set_error("tracking iteration: use_color without gt_rgb"); return NSB_ERR_ARG; }
-  }
+  if (fuse && use_color && !gt_rgb) { set_error("tracking iteration: use_color without gt_rgb"); return NSB_ERR_ARG; }
+  const FusedSeeds fs = fused_seeds(buf, 1, gt_rgb, nullptr, w_color, handle_dynamic, use_color, nullptr);
   if ((rc = forward_part(in, buf, &in2, fuse ? &fs : nullptr, stream))) return rc;
   if (!fuse && (rc = nsb_tracking_seeds(buf->depth, buf->var, buf->rgb, in->gt_depth, gt_rgb, in->n_rays, w_color, handle_dynamic, use_color,
                                         nullptr, 0, buf->g_depth, buf->g_rgb, buf->loss, seeds_scratch(buf), nsb_tracking_seeds_workspace(in->n_rays), stream))) return rc;
@@ -91,11 +93,7 @@ extern "C" int nsb_tracking_iteration_peers(const nsb_render_inputs* in, const n
   PeerX px;
   if ((rc = make_peerx(peers, &px))) return rc;
   if (in->n_rays > px.max_n) { set_error("sharded tracking iteration: %d rays exceed the exchange buffers' capacity %d", in->n_rays, px.max_n); return NSB_ERR_ARG; }
-  FusedSeeds fs; memset(&fs, 0, sizeof(fs));
-  fs.kind = 1; fs.gt_rgb = gt_rgb; fs.w_color = w_color; fs.handle_dynamic = handle_dynamic; fs.use_color = use_color;
-  fs.g_depth = buf->g_depth; fs.g_rgb = buf->g_rgb; fs.loss = buf->loss; fs.res = static_cast<double*>(seeds_scratch(buf));
-  fs.counter = seeds_counter(buf, in->n_rays);
-  fs.px = px;
+  const FusedSeeds fs = fused_seeds(buf, 1, gt_rgb, nullptr, w_color, handle_dynamic, use_color, &px);
   nsb_render_inputs in2;
   if ((rc = forward_part(in, buf, &in2, &fs, stream, true))) return rc;      // in->depth_max given: no depth-max exchange inside the forward
   PeerTail tail; tail.px = px; tail.loss = buf->loss; tail.out13 = loss_and_d_c2w;
@@ -110,12 +108,8 @@ extern "C" int nsb_mapping_iteration(const nsb_render_inputs* in, const nsb_iter
   nsb_render_inputs in2;
   const int use_color = in->stage == NSB_STAGE_COLOR;                      // Mapper.py:490
   const bool fuse = in->n_rays > 0 && in->n_rays <= NSB_INLINE_MAX_RAYS;
-  FusedSeeds fs; memset(&fs, 0, sizeof(fs));
-  if (fuse) {
-    if (use_color && !gt_rgb) { set_error("mapping iteration: colour stage without gt_rgb"); return NSB_ERR_ARG; }
-    fs.kind = 2; fs.gt_rgb = gt_rgb; fs.gt_depth_loss = gtl; fs.w_color = w_color; fs.use_color = use_color;
-    fs.g_depth = buf->g_depth; fs.g_rgb = buf->g_rgb; fs.loss = buf->loss; fs.counter = seeds_counter(buf, in->n_rays);
-  }
+  if (fuse && use_color && !gt_rgb) { set_error("mapping iteration: colour stage without gt_rgb"); return NSB_ERR_ARG; }
+  const FusedSeeds fs = fused_seeds(buf, 2, gt_rgb, gtl, w_color, 0, use_color, nullptr);
   if ((rc = forward_part(in, buf, &in2, fuse ? &fs : nullptr, stream))) return rc;
   if (!fuse && (rc = nsb_mapping_seeds(buf->depth, buf->rgb, gtl, gt_rgb, in->n_rays, w_color, use_color, buf->g_depth, buf->g_rgb, buf->loss, stream))) return rc;
   return backward_part(&in2, buf, grads, stream, nullptr, fuse);

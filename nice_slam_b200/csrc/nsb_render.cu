@@ -176,7 +176,6 @@ struct Smem {                   // carve-up of dynamic shared memory (all offset
   float* wt; uint64_t* bar; float* rays; double* far; double* zs; float* raw; double* dp; float* gocc; float* wgt;
   unsigned char* inb; float* act;
 };
-__host__ __device__ inline size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
 __host__ __device__ inline size_t smem_layout(int wbytes, int max_pts, int max_rays, int warps, int rows, bool bwd, Smem* s, unsigned char* base) {
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o = align16(o + bytes); return r; };
@@ -1077,6 +1076,13 @@ static int validate_inputs(const nsb_render_inputs* in, bool need_rays) {
   return NSB_OK;
 }
 
+// shared-memory bytes of the largest packed weight image among dec[0..n)
+static int weight_bytes(const int* dec, int n) {
+  int wb = 0;
+  for (int i = 0; i < n; i++) { const int b = packed_floats(dec[i]) * 4; wb = b > wb ? b : wb; }
+  return wb;
+}
+
 static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.in = *in;
   K.has_gt = (in->gt_depth != nullptr && in->stage != NSB_STAGE_COARSE) ? 1 : 0;    // Renderer.py:88-92
@@ -1086,9 +1092,7 @@ static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.accumulate_rays = 0;
   K.split = 1; K.group_done = nullptr; K.fwd_parts = nullptr; K.ray_parts = nullptr; K.ray_cnt = nullptr; K.tile_parts = nullptr; K.tile_rays = 0;
   memset(&K.fs, 0, sizeof(K.fs)); memset(&K.tail, 0, sizeof(K.tail));
-  int wb = 0;
-  for (int i = 0; i < K.n_dec; i++) { const int b = packed_floats(K.dec[i]) * 4; wb = b > wb ? b : wb; }
-  K.wbytes = wb;
+  K.wbytes = weight_bytes(K.dec, K.n_dec);
   K.points = nullptr; K.points_raw = nullptr; K.n_points = 0;
   K.acts_lv = in->stage == NSB_STAGE_COLOR ? 3 : -1;      // the colour decoder is the only one whose weights the mapper optimises (Mapper.py:339-341)
   memset(&K.smp, 0, sizeof(K.smp));
@@ -1147,7 +1151,6 @@ static size_t old_split_workspace_bytes(int n_rays, int S) {
 // backward = ray-gradient parts [tiles * split][kMaxTileRays][6] f64.  Items are split per decoder for batches of up to kSplitMaxPts points
 // (finer granularity for small and medium batches); larger batches evaluate all decoders of a tile in one CTA.
 constexpr long long kSplitMaxPts = 262144;
-struct TileWs { int split; int* ray_cnt; void* scratch; };
 static long long tile_count(long long n_points) { return (n_points + tc::TM - 1) / tc::TM; }
 static int tile_rays(int S) { const int r = (tc::TM - 1) / S + 2; return r < tl::kMaxTileRays ? r : tl::kMaxTileRays; }
 // Layout: [scratch ... | ray counters (N ints) at the very END of the buffer].  The counters must stay zero between launches (the completing
@@ -1159,8 +1162,9 @@ static size_t tile_scratch_bytes(int N, int S, int split, bool bwd) {
   return bwd ? (size_t)tile_count(NS) * split * tile_rays(S) * 6 * sizeof(double) : (split > 1 ? (size_t)split * NS * sizeof(float4) : 0);
 }
 static size_t tile_ws_need(int N, int S, int split, bool bwd) { return 16 + align16((size_t)N * sizeof(int)) + align16(tile_scratch_bytes(N, S, split, bwd)); }
-static bool tile_ws_plan(void* ws, size_t bytes, int N, int S, int n_dec, bool bwd, TileWs* out) {
-  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15)) return false;
+// The tile launch K in the caller's split workspace: items per tile (split), ray-completion counters, per-item scratch
+static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd) {
+  const int N = K.in.n_rays, S = K.S, n_dec = K.n_dec;
   bytes &= ~size_t(15);
   int split = ((long long)N * S <= kSplitMaxPts && n_dec > 1) ? n_dec : 1;
   if (split > 1 && g_split_model) {
@@ -1173,11 +1177,13 @@ static bool tile_ws_plan(void* ws, size_t bytes, int N, int S, int n_dec, bool b
     if (tiles >= slots && eff_one >= eff_split) split = 1;
   }
   if (bytes < tile_ws_need(N, S, split, bwd)) split = 1;
-  if (bytes < tile_ws_need(N, S, split, bwd)) return false;
-  out->split = split;
-  out->ray_cnt = reinterpret_cast<int*>(static_cast<char*>(ws) + bytes - align16((size_t)N * sizeof(int)));
-  out->scratch = static_cast<char*>(ws);
-  return true;
+  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15) || bytes < tile_ws_need(N, S, split, bwd)) {
+    set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", N, S); return NSB_ERR_ARG; }
+  K.split = split;
+  K.ray_cnt = reinterpret_cast<int*>(static_cast<char*>(ws) + bytes - align16((size_t)N * sizeof(int)));
+  if (bwd) { K.ray_parts = static_cast<double*>(ws); K.tile_rays = tile_rays(S); }
+  else K.tile_parts = split > 1 ? static_cast<float4*>(ws) : reinterpret_cast<float4*>(K.fo.raw);
+  return NSB_OK;
 }
 extern "C" size_t nsb_split_workspace_bytes(int n_rays, int S) {
   if (n_rays < 1 || S < 1) return 0;
@@ -1222,40 +1228,84 @@ static bool plan_split(KParams* K, int nd, void* ws, size_t ws_bytes) {
 
 static size_t tile_smem_bytes(bool bwd) { return tl::common_bytes(bwd) + (bwd ? sizeof(tl::BwdExtra) : 0); }
 static size_t tile_wg_smem_bytes() { return tl::kWgBytes + ((tile_smem_bytes(true) + 1023) & ~size_t(1023)) + 1024; }
-// Which tensor-core kernel family serves a launch.  mlp_backend 3: always the tile kernels; 2: always the round-1 ray-group kernels; 0 (auto): the
-// tile kernels, except that batches of up to g_small_rays rays go to the ray-group kernels (option "small_rays"; default 0 = never: since the
-// channels-last gather became straight-line code the tile kernels are level with them at 200 rays -- 0.1105 ms per tracking iteration either way,
-// r02j / r02l -- and ahead everywhere else).  Forward and backward of an iteration see the same (S, n_rays) and so pick the same family (the saved
-// ReLU bits are laid out per family).
+
+// ---- which kernel family serves a call --------------------------------------------------------------------------------------------
+// mlp_backend 3: the tile kernels; 2: the round-1 ray-group kernels; 1: FP32-FMA; 0 (auto): the tile kernels, except batches of up to
+// small_rays rays (default 0 = never: the tile kernels are level with the ray-group ones at 200 rays -- 0.1105 ms per tracking iteration
+// either way, r02j / r02l -- and ahead everywhere else).  The tile kernels take tl::kMinSamples <= S <= NSB_MAX_SAMPLES, the ray-group
+// kernels S <= kMaxPtsTc; other calls fall to FP32-FMA.  Points mode follows mlp_backend alone.  Forward and backward of an iteration see
+// the same (S, n_rays) and so pick the same family (the saved ReLU bits are laid out per family).
 static int g_small_rays = 0;
-static bool use_tile_kernels(int S, int n_rays, bool sharded) {
-  if (!(g_mlp_backend == 0 || g_mlp_backend == 3) || S < tl::kMinSamples || S > NSB_MAX_SAMPLES) return false;
-  if (g_mlp_backend == 0 && n_rays <= g_small_rays && S <= kMaxPtsTc) return false;
-  return true;
+enum class Family { Tile, Group, Fma };
+static Family kernel_family(int S, int n_rays, bool points) {
+  const bool tile_backend = g_mlp_backend == 0 || g_mlp_backend == 3;
+  if (points) return tile_backend ? Family::Tile : g_mlp_backend == 2 ? Family::Group : Family::Fma;
+  const bool small = g_mlp_backend == 0 && n_rays <= g_small_rays && S <= kMaxPtsTc;
+  if (tile_backend && S >= tl::kMinSamples && S <= NSB_MAX_SAMPLES && !small) return Family::Tile;
+  if ((g_mlp_backend == 0 || g_mlp_backend == 2) && S <= kMaxPtsTc) return Family::Group;
+  return Family::Fma;
 }
-static bool use_group_kernels(int S, int n_rays, bool sharded) {
-  return S <= kMaxPtsTc && (g_mlp_backend == 2 || (g_mlp_backend == 0 && !use_tile_kernels(S, n_rays, sharded)));
-}
+
 static bool g_attr_set[kMaxDevices] = {false};
 static int set_attrs() {
   const int dev = current_device();
   if (g_attr_set[dev]) return NSB_OK;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "fwd tc smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "bwd tc smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem_bytes(false)), "fwd tile smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_h16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem_bytes(false)), "fwd tile (f16) smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_h16_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "fwd tile (f16) carveout")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_bwd_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem_bytes(true)), "bwd tile smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_bwd_wg_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_wg_smem_bytes()), "bwd wg tile smem attr")) return NSB_ERR_CUDA;
-  // two CTAs per SM need the full shared-memory carve-out (2 x ~111 KB of the 228 KB)
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "fwd tile carveout")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_sampled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem_bytes(false)), "fwd tile (sampled) smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_tile_sampled_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "fwd tile (sampled) carveout")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_bwd_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), "bwd tile carveout")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "fwd smem attr")) return NSB_ERR_CUDA;
-  if (check_cuda(cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap), "bwd smem attr")) return NSB_ERR_CUDA;
+  // max_shared: two CTAs per SM need the full shared-memory carve-out (2 x ~111 KB of the 228 KB)
+  const struct { const void* fn; size_t smem; bool max_shared; const char* name; } attrs[] = {
+    {(const void*)render_fwd_kernel, kSmemCap, false, "render_fwd_kernel"},
+    {(const void*)render_bwd_kernel, kSmemCap, false, "render_bwd_kernel"},
+    {(const void*)render_fwd_tc_kernel, kSmemCap, false, "render_fwd_tc_kernel"},
+    {(const void*)render_bwd_tc_kernel, kSmemCap, false, "render_bwd_tc_kernel"},
+    {(const void*)render_fwd_tile_kernel, tile_smem_bytes(false), true, "render_fwd_tile_kernel"},
+    {(const void*)render_fwd_tile_h16_kernel, tile_smem_bytes(false), true, "render_fwd_tile_h16_kernel"},
+    {(const void*)render_fwd_tile_sampled_kernel, tile_smem_bytes(false), true, "render_fwd_tile_sampled_kernel"},
+    {(const void*)render_bwd_tile_kernel, tile_smem_bytes(true), true, "render_bwd_tile_kernel"},
+    {(const void*)render_bwd_wg_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_tile_kernel"},
+  };
+  for (const auto& a : attrs)
+    if (check_cuda(cudaFuncSetAttribute(a.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)a.smem), a.name) ||
+        (a.max_shared && check_cuda(cudaFuncSetAttribute(a.fn, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared), a.name)))
+      return NSB_ERR_CUDA;
   g_attr_set[dev] = true;
   return NSB_OK;
+}
+
+// ---- one launcher per family ------------------------------------------------------------------------------------------------------
+// Tile forward over n_points sample points: item = (128-point tile, decoder), two CTAs per SM.  lindisp / perturb / a given sample list take
+// the 3xTF32 instantiation with the full sampler (the others do not read K.smp); option fwd_f16 the FP16 hi|lo one.
+static int launch_tile_fwd(const KParams& K, long long n_points, cudaStream_t st) {
+  const unsigned grid = (unsigned)(tile_count(n_points) * K.split);
+  if (K.smp.lindisp || K.smp.t_rand || K.smp.z_vals) render_fwd_tile_sampled_kernel<<<grid, tl::kThreads, tile_smem_bytes(false), st>>>(K);
+  else if (g_fwd_f16) render_fwd_tile_h16_kernel<<<grid, tl::kThreads, tile_smem_bytes(false), st>>>(K);
+  else render_fwd_tile_kernel<<<grid, tl::kThreads, tile_smem_bytes(false), st>>>(K);
+  return check_cuda(cudaGetLastError(), K.points ? "render_fwd_tile_kernel(points) launch" : "render_fwd_tile_kernel launch");
+}
+// Round-1 ray-group kernels: 512 threads, <= 2 tiles of 128 points per CTA, decoder-parallel CTAs when plan_split finds them faster
+static int launch_group(KParams K, bool bwd, void* ws, size_t ws_bytes, cudaStream_t st) {
+  int warps; size_t smem;
+  choose_config(K.in.n_rays, K.S, bwd ? kRowsBwd : kRowsFwd, bwd, K.wbytes, 8, &K, &warps, &smem, kMaxPtsTc);
+  plan_split(&K, K.n_dec, ws, ws_bytes);
+  const int grid = ((K.in.n_rays + K.rays_per_block - 1) / K.rays_per_block) * K.split;
+  const size_t smem_tc = tc_total_smem(K.max_pts, K.max_rays, bwd);
+  if (smem_tc > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem_tc); return NSB_ERR_UNSUPPORTED; }
+  if (bwd) render_bwd_tc_kernel<<<grid, tc::kThreads, smem_tc, st>>>(K);
+  else render_fwd_tc_kernel<<<grid, tc::kThreads, smem_tc, st>>>(K);
+  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_tc_kernel launch" : "render_fwd_tc_kernel launch");
+}
+// FP32-FMA kernels: CTA geometry and weight-image size for the decoders of K
+static int fma_config(KParams& K, bool bwd, int* warps, size_t* smem) {
+  K.wbytes = weight_bytes(K.dec, K.n_dec);
+  choose_config(K.in.n_rays, K.S, bwd ? kRowsBwd : kRowsFwd, bwd, K.wbytes, 8, &K, warps, smem);
+  if (*smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", *smem); return NSB_ERR_UNSUPPORTED; }
+  return NSB_OK;
+}
+static int launch_fma(KParams K, bool bwd, cudaStream_t st) {
+  int warps; size_t smem;
+  const int rc = fma_config(K, bwd, &warps, &smem); if (rc) return rc;
+  const int grid = (K.in.n_rays + K.rays_per_block - 1) / K.rays_per_block;
+  if (bwd) render_bwd_kernel<<<grid, warps * 32, smem, st>>>(K);
+  else render_fwd_kernel<<<grid, warps * 32, smem, st>>>(K);
+  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_kernel launch" : "render_fwd_kernel launch");
 }
 
 }  // namespace nsb
@@ -1299,43 +1349,20 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
   KParams K; fill_common(K, in); K.fo = *out; memset(&K.bw, 0, sizeof(K.bw));
   if ((rc = apply_sampling(K, smp))) return rc;
   if (fs != nullptr) K.fs = *fs;
-  const bool sharded = fs != nullptr && fs->px.world > 1;
-  const bool tile = use_tile_kernels(K.S, in->n_rays, sharded), group = use_group_kernels(K.S, in->n_rays, sharded);
-  if (!tile && !group) K.fo.masks = nullptr;                      // only the tensor-core forwards produce masks
+  const Family fam = kernel_family(K.S, in->n_rays, false);
+  if (fam == Family::Fma) K.fo.masks = nullptr;                   // only the tensor-core forwards produce masks
   if (K.S > NSB_MAX_SAMPLES) { set_error("n_samples+n_surface = %d exceeds %d", K.S, NSB_MAX_SAMPLES); return NSB_ERR_UNSUPPORTED; }
   if (K.has_gt && in->n_surface > 0 && !in->t_surface) { set_error("t_surface NULL"); return NSB_ERR_ARG; }
   if ((rc = set_attrs())) return rc;
-  if (K.fs.px.world > 1 && !((tile || group) && in->gt_depth != nullptr)) {
+  if (K.fs.px.world > 1 && !(fam != Family::Fma && in->gt_depth != nullptr)) {
     set_error("in-kernel exchanges of a sharded forward need a tensor-core back-end and <= %d rays per rank", NSB_INLINE_MAX_RAYS); return NSB_ERR_UNSUPPORTED; }
-  if (tile) {                                             // tile kernels: item = (128-point tile, decoder), two CTAs per SM
+  if (fam == Family::Tile) {
     if (!out->z_vals || !out->raw) { set_error("the tensor-core forward needs z_vals and raw outputs"); return NSB_ERR_ARG; }
-    TileWs w;
-    if (!tile_ws_plan(out->split_workspace, out->split_workspace_bytes, in->n_rays, K.S, K.n_dec, false, &w)) {
-      set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", in->n_rays, K.S); return NSB_ERR_ARG; }
-    K.split = w.split; K.ray_cnt = w.ray_cnt;
-    K.tile_parts = w.split > 1 ? static_cast<float4*>(w.scratch) : reinterpret_cast<float4*>(out->raw);
-    const long long grid_t = tile_count((long long)in->n_rays * K.S) * K.split;
-    // lindisp / perturb / a given sample list: the 3xTF32 instantiation with the full sampler (the default one does not read K.smp)
-    if (K.smp.lindisp || K.smp.t_rand || K.smp.z_vals) render_fwd_tile_sampled_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
-    else if (g_fwd_f16) render_fwd_tile_h16_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
-    else render_fwd_tile_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
-    return check_cuda(cudaGetLastError(), "render_fwd_tile_kernel launch");
+    if ((rc = plan_tile_ws(K, out->split_workspace, out->split_workspace_bytes, false))) return rc;
+    return launch_tile_fwd(K, (long long)in->n_rays * K.S, (cudaStream_t)stream);
   }
-  int warps; size_t smem;
-  choose_config(in->n_rays, K.S, kRowsFwd, false, K.wbytes, 8, &K, &warps, &smem);
-  if (smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem); return NSB_ERR_UNSUPPORTED; }
-  const int grid = (in->n_rays + K.rays_per_block - 1) / K.rays_per_block;
-  if (group) {                                            // tensor-core decoders, 512 threads, <= 2 tiles of 128 points per CTA
-    choose_config(in->n_rays, K.S, kRowsFwd, false, K.wbytes, 8, &K, &warps, &smem, kMaxPtsTc);
-    plan_split(&K, K.n_dec, out->split_workspace, out->split_workspace_bytes);
-    const int grid_tc = ((in->n_rays + K.rays_per_block - 1) / K.rays_per_block) * K.split;
-    const size_t smem_tc = tc_total_smem(K.max_pts, K.max_rays);
-    if (smem_tc > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem_tc); return NSB_ERR_UNSUPPORTED; }
-    render_fwd_tc_kernel<<<grid_tc, tc::kThreads, smem_tc, (cudaStream_t)stream>>>(K);
-    return check_cuda(cudaGetLastError(), "render_fwd_tc_kernel launch");
-  }
-  render_fwd_kernel<<<grid, warps * 32, smem, (cudaStream_t)stream>>>(K);
-  return check_cuda(cudaGetLastError(), "render_fwd_kernel launch");
+  if (fam == Family::Group) return launch_group(K, false, out->split_workspace, out->split_workspace_bytes, (cudaStream_t)stream);
+  return launch_fma(K, false, (cudaStream_t)stream);
 }
 
 extern "C" int nsb_eval_points(const nsb_render_inputs* in, const double* points, int n_points, float* raw, void* stream) {
@@ -1355,13 +1382,9 @@ extern "C" int nsb_eval_points(const nsb_render_inputs* in, const double* points
   const size_t smem = smem_layout(K.wbytes, ppb, 1, warps, kRowsFwd, false, nullptr, nullptr);
   K.rays_per_block = ppb; K.max_pts = ppb; K.max_rays = 1;
   const int grid = (n_points + ppb - 1) / ppb;
-  if (g_mlp_backend == 0 || g_mlp_backend == 3) {
-    K.split = 1;
-    if (g_fwd_f16) render_fwd_tile_h16_kernel<<<(unsigned)tile_count(n_points), tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
-    else render_fwd_tile_kernel<<<(unsigned)tile_count(n_points), tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K);
-    return check_cuda(cudaGetLastError(), "render_fwd_tile_kernel(points) launch");
-  }
-  if (g_mlp_backend == 2) {
+  const Family fam = kernel_family(K.S, 0, true);
+  if (fam == Family::Tile) return launch_tile_fwd(K, n_points, (cudaStream_t)stream);
+  if (fam == Family::Group) {
     render_fwd_tc_kernel<<<grid, tc::kThreads, tc_total_smem(K.max_pts, K.max_rays), (cudaStream_t)stream>>>(K);
     return check_cuda(cudaGetLastError(), "render_fwd_tc_kernel(points) launch");
   }
@@ -1421,96 +1444,65 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   // grids/weights that are not part of this stage get no gradient
   for (int l = 0; l < 4; l++) { bool used = false; for (int i = 0; i < K.n_dec; i++) used |= K.dec[i] == l; if (!used) { K.bw.d_grid[l] = nullptr; } }
   if ((rc = set_attrs())) return rc;
+  // Every launch below starts from K, so each carries the FP32-FMA geometry of the whole stage (only the FP32-FMA kernels read it).
   int warps; size_t smem;
-  choose_config(in->n_rays, K.S, kRowsBwd, true, K.wbytes, 8, &K, &warps, &smem);
-  if (smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem); return NSB_ERR_UNSUPPORTED; }
+  if ((rc = fma_config(K, true, &warps, &smem))) return rc;
+  // Plan: with the saved ReLU masks a tensor-core launch for the decoders that only need input gradients (rays, voxels), then one for those
+  // whose WEIGHT gradients are requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341): on the tensor cores when the
+  // forward kept its layer outputs (acts; one item per tile, one CTA per SM), else FP32-FMA, which recomputes the forward.  Without masks,
+  // or on the FP32-FMA back-end, one FP32-FMA launch for every decoder.
+  enum Kind { TileIg, GroupIg, WgTile, Fma };
+  const Family fam = kernel_family(K.S, in->n_rays, false);
   const bool sharded = tail != nullptr && tail->px.world > 1;
-  const bool tile = use_tile_kernels(K.S, in->n_rays, sharded), group = use_group_kernels(K.S, in->n_rays, sharded);
-  if (bw->masks != nullptr && (group || tile)) {                  // (no saved ReLU masks -> FP32 kernel, which recomputes the forward)
-    // Tensor-core kernel for the decoders that only need input gradients (rays, voxels).  Decoders whose WEIGHT gradients are
-    // requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341) go through the FP32-FMA kernel in a second
-    // launch that adds its share of the ray gradients.
-    KParams T = K;
-    T.n_dec = 0;
-    int n_w = 0, wdec[3], wpos[3];
+  KParams L[2]; Kind kind[2]; int n = 0;
+  if (bw->masks == nullptr || fam == Family::Fma) { L[n] = K; kind[n++] = Fma; }
+  else {
+    KParams ig = K, wg = K;
+    ig.n_dec = wg.n_dec = 0;
     for (int i = 0; i < K.n_dec; i++) {
-      if (bw->d_flat[K.dec[i]] != nullptr) { wdec[n_w] = K.dec[i]; wpos[n_w] = i; n_w++; }
-      else { T.dec[T.n_dec] = K.dec[i]; T.dec_pos[T.n_dec] = i; T.n_dec++; }
+      KParams& P = bw->d_flat[K.dec[i]] != nullptr ? wg : ig;
+      P.dec[P.n_dec] = K.dec[i]; P.dec_pos[P.n_dec] = i; P.n_dec++;
     }
-    // Weight gradients on the tensor cores: the colour decoder, when the forward kept its layer outputs (acts) -- a second tile launch with one item
-    // per tile (one CTA per SM) after the input-gradient launch of the other decoders; it adds its share of the ray gradients.
-    const bool wg_tc = n_w == 1 && wdec[0] == 3 && bw->acts != nullptr && tile && g_wgrad_tc && !sharded;
-    if (T.n_dec > 0) {
-      if (n_w == 0 && want_pose) T.bw.pose_dirs = bw->pose_dirs;   // the tensor-core launch is the last writer of the ray gradients
-      if (tile) {
-        TileWs w;
-        if (!tile_ws_plan(bw->split_workspace, bw->split_workspace_bytes, in->n_rays, T.S, T.n_dec, true, &w)) {
-          set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", in->n_rays, T.S); return NSB_ERR_ARG; }
-        T.split = w.split; T.ray_cnt = w.ray_cnt; T.ray_parts = static_cast<double*>(w.scratch); T.tile_rays = tile_rays(T.S);
-        if (tail != nullptr && tail->px.world > 1) {
-          if (n_w != 0 || T.bw.pose_dirs == nullptr) { set_error("sharded backward tail needs pose_dirs and no decoder weight gradients"); return NSB_ERR_ARG; }
-          T.tail = *tail;
-        }
-        const long long grid_t = tile_count((long long)in->n_rays * T.S) * T.split;
-        if (after_forward && !any_w && g_pdl) {
-          // Programmatic dependent launch: the forward kernel signals `launch_dependents` when it starts, so this grid's CTAs become resident as
-          // forward CTAs retire and run their set-up (accumulator slot, barrier init, first weight units through TMA) under the forward's tail
-          // (ray compositing, the last CTA's loss seeds / peer exchange); `griddepcontrol.wait` in front of the first read of a forward
-          // result holds them until the forward grid has completed and flushed.
-          cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-          cfg.gridDim = dim3((unsigned)grid_t); cfg.blockDim = dim3(tl::kThreads); cfg.dynamicSmemBytes = tile_smem_bytes(true); cfg.stream = st;
-          cudaLaunchAttribute at[1];
-          at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-          cfg.attrs = at; cfg.numAttrs = 1;
-          if ((rc = check_cuda(cudaLaunchKernelEx(&cfg, render_bwd_tile_kernel, T), "render_bwd_tile_kernel launch (dependent)"))) return rc;
-        } else {
-          render_bwd_tile_kernel<<<(unsigned)grid_t, tl::kThreads, tile_smem_bytes(true), st>>>(T);
-          if ((rc = check_cuda(cudaGetLastError(), "render_bwd_tile_kernel launch"))) return rc;
-        }
-      } else {
-      if (tail != nullptr && tail->px.world > 1) {
-        if (n_w != 0 || T.bw.pose_dirs == nullptr) { set_error("sharded backward tail needs pose_dirs and no decoder weight gradients"); return NSB_ERR_ARG; }
-        T.tail = *tail;
-      }
-      choose_config(in->n_rays, T.S, kRowsBwd, true, T.wbytes, 8, &T, &warps, &smem, kMaxPtsTc);
-      plan_split(&T, T.n_dec, bw->split_workspace, bw->split_workspace_bytes);
-      const int grid_tc = ((in->n_rays + T.rays_per_block - 1) / T.rays_per_block) * T.split;
-      const size_t smem_tc = tc_total_smem(T.max_pts, T.max_rays, true);
-      if (smem_tc > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem_tc); return NSB_ERR_UNSUPPORTED; }
-      render_bwd_tc_kernel<<<grid_tc, tc::kThreads, smem_tc, st>>>(T);
-      if ((rc = check_cuda(cudaGetLastError(), "render_bwd_tc_kernel launch"))) return rc;
-      }
-      if (n_w == 0) return NSB_OK;
-      K.accumulate_rays = 1;
-    }
-    if (wg_tc) {
-      KParams W = K;
-      W.n_dec = 1; W.dec[0] = wdec[0]; W.dec_pos[0] = wpos[0];
-      W.accumulate_rays = T.n_dec > 0 ? 1 : 0;
-      W.bw.pose_dirs = want_pose ? bw->pose_dirs : nullptr;          // last writer of the ray gradients: d c2w by its last CTA
-      TileWs w;
-      if (!tile_ws_plan(bw->split_workspace, bw->split_workspace_bytes, in->n_rays, W.S, 1, true, &w)) {
-        set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", in->n_rays, W.S); return NSB_ERR_ARG; }
-      W.split = 1; W.ray_cnt = w.ray_cnt; W.ray_parts = static_cast<double*>(w.scratch); W.tile_rays = tile_rays(W.S);
-      render_bwd_wg_tile_kernel<<<(unsigned)tile_count((long long)in->n_rays * W.S), tl::kThreads, tile_wg_smem_bytes(), st>>>(W);
-      if ((rc = check_cuda(cudaGetLastError(), "render_bwd_wg_tile_kernel launch"))) return rc;
-      return launch_unpack_grads(W.d_packed, bw->d_flat, st);
-    }
-    if (T.n_dec > 0) {
-      K.n_dec = n_w;
-      for (int i = 0; i < n_w; i++) { K.dec[i] = wdec[i]; K.dec_pos[i] = wpos[i]; }
-      int wb = 0;
-      for (int i = 0; i < K.n_dec; i++) { const int b = packed_floats(K.dec[i]) * 4; wb = b > wb ? b : wb; }
-      K.wbytes = wb;
-      choose_config(in->n_rays, K.S, kRowsBwd, true, K.wbytes, 8, &K, &warps, &smem);
-      if (smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem); return NSB_ERR_UNSUPPORTED; }
-    }
+    if (ig.n_dec > 0) { L[n] = ig; kind[n++] = fam == Family::Tile ? TileIg : GroupIg; }
+    const bool wg_tc = wg.n_dec == 1 && wg.dec[0] == NSB_COLOR && bw->acts != nullptr && fam == Family::Tile && g_wgrad_tc && !sharded;
+    if (wg.n_dec > 0) { L[n] = wg; kind[n++] = wg_tc ? WgTile : Fma; }       // (every decoder here: wg == K)
   }
-  const int grid = (in->n_rays + K.rays_per_block - 1) / K.rays_per_block;
-  render_bwd_kernel<<<grid, warps * 32, smem, st>>>(K);
-  if ((rc = check_cuda(cudaGetLastError(), "render_bwd_kernel launch"))) return rc;
+  // Every launch after the first adds to the ray gradients; the last one writes d c2w from its last CTA (the FP32-FMA kernel does not:
+  // a separate nsb_pose_grad launch follows it).  A sharded tail is summed by the last CTA of a tensor-core input-gradient launch.
+  for (int i = 1; i < n; i++) L[i].accumulate_rays = 1;
+  if (kind[n - 1] != Fma) L[n - 1].bw.pose_dirs = bw->pose_dirs;
+  if (sharded && (kind[0] == TileIg || kind[0] == GroupIg)) {
+    if (n > 1 || !want_pose) { set_error("sharded backward tail needs pose_dirs and no decoder weight gradients"); return NSB_ERR_ARG; }
+    L[0].tail = *tail;
+  }
+  for (int i = 0; i < n; i++) {
+    KParams& P = L[i];
+    const unsigned tiles = (unsigned)tile_count((long long)in->n_rays * P.S);
+    if (kind[i] == GroupIg) rc = launch_group(P, true, bw->split_workspace, bw->split_workspace_bytes, st);
+    else if (kind[i] == Fma) rc = launch_fma(P, true, st);
+    else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true))) return rc;
+    else if (kind[i] == WgTile) {
+      render_bwd_wg_tile_kernel<<<tiles, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
+      rc = check_cuda(cudaGetLastError(), "render_bwd_wg_tile_kernel launch");
+    } else if (after_forward && !any_w && g_pdl) {
+      // Programmatic dependent launch: the forward kernel signals `launch_dependents` when it starts, so this grid's CTAs become resident as
+      // forward CTAs retire and run their set-up (accumulator slot, barrier init, first weight units through TMA) under the forward's tail
+      // (ray compositing, the last CTA's loss seeds / peer exchange); `griddepcontrol.wait` in front of the first read of a forward
+      // result holds them until the forward grid has completed and flushed.
+      cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
+      cfg.gridDim = dim3(tiles * P.split); cfg.blockDim = dim3(tl::kThreads); cfg.dynamicSmemBytes = tile_smem_bytes(true); cfg.stream = st;
+      cudaLaunchAttribute at[1];
+      at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+      cfg.attrs = at; cfg.numAttrs = 1;
+      rc = check_cuda(cudaLaunchKernelEx(&cfg, render_bwd_tile_kernel, P), "render_bwd_tile_kernel launch (dependent)");
+    } else {
+      render_bwd_tile_kernel<<<tiles * P.split, tl::kThreads, tile_smem_bytes(true), st>>>(P);
+      rc = check_cuda(cudaGetLastError(), "render_bwd_tile_kernel launch");
+    }
+    if (rc) return rc;
+  }
   if (any_w && (rc = launch_unpack_grads(K.d_packed, bw->d_flat, st))) return rc;
-  if (want_pose) {                                                 // FP32 path: separate launches
+  if (kind[n - 1] == Fma && want_pose) {
     if ((rc = nsb_pose_grad(bw->pose_dirs, bw->d_rays_o, bw->d_rays_d, in->n_rays, bw->d_c2w, stream))) return rc;
     if (bw->result_dst != nullptr) return nsb_copy_block(bw->result_dst, bw->result_src, bw->result_bytes, stream);
   }

@@ -9,6 +9,7 @@ reference package is not importable.  It holds parameters only; evaluation alway
 import torch
 import torch.nn as nn
 
+from . import _lib
 from ._lib import LEVELS
 
 HIDDEN, EMBED, C_DIM = 32, 93, 32
@@ -79,3 +80,24 @@ def named_params(decoders, level_name):
     if "embedder._B" not in out and hasattr(sub, "embedder") and hasattr(sub.embedder, "_B"):
         out["embedder._B"] = sub.embedder._B          # non-learnable variant keeps _B as a plain tensor
     return out
+
+
+def decoder_params_struct(decoders, level_name):
+    """nsb_decoder_params of one decoder (pointers into the live nn.Parameters)."""
+    p = named_params(decoders, level_name)
+    li = LEVELS.index(level_name)
+    dp = _lib.DecoderParams()
+    for t in p.values():
+        if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous():
+            raise RuntimeError("nice_slam_b200: decoder parameters must be contiguous float32 CUDA tensors")
+    if li != 0:
+        dp.B = p["embedder._B"].data_ptr()
+    for i in range(5):
+        dp.W[i] = p["pts_linears.%d.weight" % i].data_ptr()
+        dp.b[i] = p["pts_linears.%d.bias" % i].data_ptr()
+        if li != 0:
+            dp.Wc[i] = p["fc_c.%d.weight" % i].data_ptr()
+            dp.bc[i] = p["fc_c.%d.bias" % i].data_ptr()
+    dp.Wo = p["output_linear.weight"].data_ptr()
+    dp.bo = p["output_linear.bias"].data_ptr()
+    return dp

@@ -130,23 +130,10 @@ class ShardedTrackingIteration:
         draws).  The batch depth maxima (Renderer.py:109,144) are then reduced locally over the full list (one tiny launch) and the iteration keeps
         only the two exchanges that sit at kernel tails (median pool, [loss | d c2w] sum); without it every forward CTA first waits for all ranks'
         shard maxima -- which exposes the launch skew between the ranks' independent graph replays."""
-        from . import _lib
-        from .renderer import _inputs, _linspaces
         x = self.ctx
-        ro, rd, gd, gc = x.device_views()
-        call, grids, _ = x.r._call(c, decoders, x.stage, gd, x.dev)
-        t_u, t_s = _linspaces(x.r.N_samples, x.r.N_surface, x.dev)
-        inp = _inputs(call, ro, rd, x.depth_max, t_u, t_s, [g.detach() for g in grids])
-        fo = _lib.ForwardOutputs(x.depth.data_ptr(), x.var.data_ptr(), x.rgb.data_ptr(), x.z_vals.data_ptr(), x.raw.data_ptr(), None,
-                                 x.masks.data_ptr(), x.split_ws.data_ptr() if x.split_bytes else None, x.split_bytes,
-                                 x.acts.data_ptr() if x.acts is not None else None)
-        bw = x._grads(c)
-        bw.acts = x.acts.data_ptr() if x.acts is not None else None
-        if x.split_bytes:
-            bw.split_workspace, bw.split_workspace_bytes = x.split_ws.data_ptr(), x.split_bytes
-        bw.z_vals, bw.raw, bw.g_depth, bw.g_rgb, bw.masks = (x.z_vals.data_ptr(), x.raw.data_ptr(), x.g_depth.data_ptr(),
-                                                              x.g_rgb.data_ptr(), x.masks.data_ptr())
-        self._p = dict(call=call, grids=grids, lin=(t_u, t_s), inp=inp, fo=fo, bw=bw, dirs=dirs, gd=gd, gc=gc,
+        _, _, gd, gc = x.device_views()
+        call, grids, inp, fo, bw = x.render_structs(c, decoders)
+        self._p = dict(call=call, grids=grids, inp=inp, fo=fo, bw=bw, dirs=dirs, gd=gd, gc=gc,
                        w_color=w_color, hd=int(handle_dynamic), uc=int(use_color), ggd=global_gt_depth)
 
     def enqueue(self, out13_ptr=None):
@@ -264,24 +251,11 @@ class ShardedMappingIteration:
         """global_gt_depth: the sensor depths of the WHOLE batch (every rank samples the same window pixels from replicated keyframes, so it
         has them): the batch depth maxima (Renderer.py:109,144) are then computed locally on the full batch before sharding and the iteration
         needs exactly ONE collective, the all-reduce of the packed gradient block (SURVEY.md 8e).  None: MAX all-reduce of the shard maxima."""
-        from . import _lib
-        from .renderer import _inputs, _linspaces
         x = self.ctx
-        ro, rd, gd, gc = x.device_views()
-        call, grids, _ = x.r._call(c, decoders, x.stage, gd if x.render_with_depth else None, x.dev)
-        t_u, t_s = _linspaces(x.r.N_samples, x.r.N_surface, x.dev)
-        inp = _inputs(call, ro, rd, x.depth_max, t_u, t_s, [g.detach() for g in grids])
-        fo = _lib.ForwardOutputs(x.depth.data_ptr(), x.var.data_ptr(), x.rgb.data_ptr(), x.z_vals.data_ptr(), x.raw.data_ptr(), None,
-                                 x.masks.data_ptr(), x.split_ws.data_ptr() if x.split_bytes else None, x.split_bytes,
-                                 x.acts.data_ptr() if x.acts is not None else None)
-        bw = x._grads(c)
-        bw.acts = x.acts.data_ptr() if x.acts is not None else None
-        if x.split_bytes:
-            bw.split_workspace, bw.split_workspace_bytes = x.split_ws.data_ptr(), x.split_bytes
-        bw.z_vals, bw.raw, bw.g_depth, bw.g_rgb, bw.masks = (x.z_vals.data_ptr(), x.raw.data_ptr(), x.g_depth.data_ptr(),
-                                                              x.g_rgb.data_ptr(), x.masks.data_ptr())
+        _, _, gd, gc = x.device_views()
+        call, grids, inp, fo, bw = x.render_structs(c, decoders)
         bw.workspace = x.bwd_ws.data_ptr()
-        self._p = dict(call=call, grids=grids, lin=(t_u, t_s), inp=inp, fo=fo, bw=bw, dirs=dirs, offs=frame_offsets, gd=gd, gc=gc,
+        self._p = dict(call=call, grids=grids, inp=inp, fo=fo, bw=bw, dirs=dirs, offs=frame_offsets, gd=gd, gc=gc,
                        w_color=w_color, uc=int(x.stage == "color"), ggd=global_gt_depth)
         self.collectives_per_step = (1 if (global_gt_depth is not None or not x.render_with_depth) else 2) if world()[1] > 1 else 0
 

@@ -9,29 +9,8 @@ import torch
 
 from . import _lib
 from ._lib import LEVELS
-from .decoders import named_params
+from .decoders import decoder_params_struct, named_params
 from .renderer import _VP, _stream, grid_struct
-
-
-def decoder_params_struct(decoders, level_name):
-    """nsb_decoder_params of one decoder (pointers into the live nn.Parameters)."""
-    p = named_params(decoders, level_name)
-    li = LEVELS.index(level_name)
-    dp = _lib.DecoderParams()
-    for t in p.values():
-        if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous():
-            raise RuntimeError("nice_slam_b200: decoder parameters must be contiguous float32 CUDA tensors")
-    if li != 0:
-        dp.B = p["embedder._B"].data_ptr()
-    for i in range(5):
-        dp.W[i] = p["pts_linears.%d.weight" % i].data_ptr()
-        dp.b[i] = p["pts_linears.%d.bias" % i].data_ptr()
-        if li != 0:
-            dp.Wc[i] = p["fc_c.%d.weight" % i].data_ptr()
-            dp.bc[i] = p["fc_c.%d.bias" % i].data_ptr()
-    dp.Wo = p["output_linear.weight"].data_ptr()
-    dp.bo = p["output_linear.bias"].data_ptr()
-    return dp
 
 
 class FusedMapperAdam:

@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from ._lib import LEVELS, STAGES, STAGE_DECODERS
-from .decoders import named_params
+from .decoders import decoder_params_struct, named_params
 
 _VP = C.c_void_p
 
@@ -79,22 +79,7 @@ class _PackCache:
             keep = []
             for lvl, key in need:
                 li = LEVELS.index(lvl)
-                p = params[lvl]
-                dp = _lib.DecoderParams()
-                for t in p.values():
-                    _require_cuda(t, "decoder parameter")
-                    if t.dtype != torch.float32 or not t.is_contiguous():
-                        raise RuntimeError("decoder parameters must be contiguous float32")
-                if li != 0:
-                    dp.B = p["embedder._B"].data_ptr()
-                for i in range(5):
-                    dp.W[i] = p["pts_linears.%d.weight" % i].data_ptr()
-                    dp.b[i] = p["pts_linears.%d.bias" % i].data_ptr()
-                    if li != 0:
-                        dp.Wc[i] = p["fc_c.%d.weight" % i].data_ptr()
-                        dp.bc[i] = p["fc_c.%d.bias" % i].data_ptr()
-                dp.Wo = p["output_linear.weight"].data_ptr()
-                dp.bo = p["output_linear.bias"].data_ptr()
+                dp = decoder_params_struct(decoders, lvl)
                 buf = torch.empty(L.nsb_packed_decoder_floats(li), dtype=torch.float32, device=device)
                 keep.append(dp)
                 arr_p[li] = C.pointer(dp)
@@ -166,9 +151,10 @@ def _samples_per_ray(call):
     return call.n_samples + (call.n_surface if has_gt else 0)
 
 
-def _forward_only(call, ro, rd, grids):
-    """The render forward without autograd and without the state a backward would need (saved ReLU masks, layer outputs):
-    the first pass of hierarchical sampling.  Returns z_vals [N,S] f64 and raw [N,S,4]."""
+def _forward_setup(call, ro):
+    """What both forwards set up for a batch: the batch depth maxima (only above INLINE_MAX_RAYS rays: smaller batches are reduced inside
+    the render kernel), the linspaces, the outputs and the split workspace.  Returns (depth_max, t_u, t_s, outputs, ForwardOutputs) with
+    outputs = (depth, var, rgb, z_vals, raw, split); the struct has no corner_idx, masks or acts."""
     L = _lib.lib()
     dev = ro.device
     n = ro.shape[0]
@@ -178,7 +164,6 @@ def _forward_only(call, ro, rd, grids):
         depth_max = torch.empty(2, dtype=torch.float32, device=dev)
         _lib.check(L.nsb_batch_max_depth(_ptr(call.gt_depth), n, _ptr(depth_max), _stream()), "nsb_batch_max_depth")
     t_u, t_s = _linspaces(call.n_samples, call.n_surface, dev)
-    inp = _inputs(call, ro, rd, depth_max, t_u, t_s, grids)
     depth = torch.empty(n, dtype=torch.float64, device=dev)
     var = torch.empty(n, dtype=torch.float64, device=dev)
     rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
@@ -188,8 +173,16 @@ def _forward_only(call, ro, rd, grids):
     split = torch.zeros(nsplit, dtype=torch.uint8, device=dev) if nsplit else None
     out = _lib.ForwardOutputs(depth.data_ptr(), var.data_ptr(), rgb.data_ptr(), z_vals.data_ptr(), raw.data_ptr(), None, None,
                               split.data_ptr() if nsplit else None, nsplit, None)
-    if n > 0:
-        _lib.check(L.nsb_render_forward_sampled(C.byref(inp), _sampling(call), C.byref(out), _stream()), "nsb_render_forward_sampled")
+    return depth_max, t_u, t_s, (depth, var, rgb, z_vals, raw, split), out
+
+
+def _forward_only(call, ro, rd, grids):
+    """The render forward without autograd and without the state a backward would need (saved ReLU masks, layer outputs):
+    the first pass of hierarchical sampling.  Returns z_vals [N,S] f64 and raw [N,S,4]."""
+    depth_max, t_u, t_s, (_, _, _, z_vals, raw, _), out = _forward_setup(call, ro)
+    inp = _inputs(call, ro, rd, depth_max, t_u, t_s, grids)
+    if ro.shape[0] > 0:
+        _lib.check(_lib.lib().nsb_render_forward_sampled(C.byref(inp), _sampling(call), C.byref(out), _stream()), "nsb_render_forward_sampled")
     return z_vals, raw
 
 
@@ -206,24 +199,14 @@ class _RenderFn(torch.autograd.Function):
         ro = rays_o.detach().contiguous().float()
         rd = rays_d.detach().contiguous().float()
         n = ro.shape[0]
-        S = _samples_per_ray(call)
-        depth_max = None
-        if call.gt_depth is not None and n > INLINE_MAX_RAYS:             # smaller batches: the render kernel reduces gt_depth itself
-            depth_max = torch.empty(2, dtype=torch.float32, device=dev)
-            _lib.check(L.nsb_batch_max_depth(_ptr(call.gt_depth), n, _ptr(depth_max), _stream()), "nsb_batch_max_depth")
-        t_u, t_s = _linspaces(call.n_samples, call.n_surface, dev)
+        depth_max, t_u, t_s, (depth, var, rgb, z_vals, raw, split), out = _forward_setup(call, ro)
+        S = z_vals.shape[1]
         # a grid argument is either the grid itself or, for a frustum-masked grid (see FusedRenderer._masked_leaf), the mapper's 1-D leaf
         # `val_grad`; the data the kernels read is always the full grid
         data = [call.grid_data[j] if call.masked[j] is not None else grids[j].detach() for j in range(n_lvl)]
         inp = _inputs(call, ro, rd, depth_max, t_u, t_s, data)
-        depth = torch.empty(n, dtype=torch.float64, device=dev)
-        var = torch.empty(n, dtype=torch.float64, device=dev)
-        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        z_vals = torch.empty(n, S, dtype=torch.float64, device=dev)
-        raw = torch.empty(n, S, 4, dtype=torch.float32, device=dev)
         masks = torch.empty(n, S, 15, dtype=torch.int32, device=dev)      # ReLU sign bits: lets backward skip the forward recompute
-        nsplit = L.nsb_split_workspace_bytes(n, S)                        # small batches: one CTA per (ray group, decoder)
-        split = torch.zeros(nsplit, dtype=torch.uint8, device=dev) if nsplit else None
+        out.masks = masks.data_ptr()
         # colour-decoder parameters that need a gradient (the mapper's colour stage, Mapper.py:339-341): keep the decoder's layer outputs so that
         # the backward computes the weight gradients on the tensor cores
         acts = None
@@ -231,8 +214,7 @@ class _RenderFn(torch.autograd.Function):
             k0 = 3 + n_lvl + sum(len(call.param_names[l]) for l in call.levels[: call.levels.index("color")])
             if any(ctx.needs_input_grad[k0 + i] for i in range(len(call.param_names["color"]))):
                 acts = torch.empty(n, S, 5, 32, dtype=torch.float32, device=dev)
-        out = _lib.ForwardOutputs(depth.data_ptr(), var.data_ptr(), rgb.data_ptr(), z_vals.data_ptr(), raw.data_ptr(), None, masks.data_ptr(),
-                                  split.data_ptr() if nsplit else None, nsplit, acts.data_ptr() if acts is not None else None)
+                out.acts = acts.data_ptr()
         corner = None
         if call.aux is not None:
             corner = torch.empty(n, S, 3, dtype=torch.int32, device=dev)

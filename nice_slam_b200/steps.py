@@ -141,6 +141,24 @@ class IterationContext:
         self.zero_grads()
         return bw
 
+    def render_structs(self, c, decoders):
+        """(call, grids, RenderInputs, ForwardOutputs, BackwardArgs) of a render over the context's device inputs (device_views) and
+        buffers, for the split-phase forms that call the render entry points one by one (dist.py).  Keep call and grids alive while the
+        structs are used: they own the packed decoders the inputs point at.  (Re)zeroes the accumulation buffers."""
+        ro, rd, gd, _ = self.device_views()
+        call, grids, _ = self.r._call(c, decoders, self.stage, gd if self.render_with_depth else None, self.dev)
+        t_u, t_s = _linspaces(self.r.N_samples, self.r.N_surface, self.dev)
+        inp = _inputs(call, ro, rd, self.depth_max, t_u, t_s, [g.detach() for g in grids])
+        acts = self.acts.data_ptr() if self.acts is not None else None
+        split = self.split_ws.data_ptr() if self.split_bytes else None
+        fo = _lib.ForwardOutputs(self.depth.data_ptr(), self.var.data_ptr(), self.rgb.data_ptr(), self.z_vals.data_ptr(), self.raw.data_ptr(), None,
+                                 self.masks.data_ptr(), split, self.split_bytes, acts)
+        bw = self._grads(c)
+        bw.z_vals, bw.raw, bw.g_depth, bw.g_rgb, bw.masks = (self.z_vals.data_ptr(), self.raw.data_ptr(), self.g_depth.data_ptr(),
+                                                              self.g_rgb.data_ptr(), self.masks.data_ptr())
+        bw.split_workspace, bw.split_workspace_bytes, bw.acts = split, self.split_bytes, acts
+        return call, grids, inp, fo, bw
+
     def zero_grads(self):
         if self.packed.numel() > 4:
             self.packed.zero_()                                   # one memset: loss slot, keyframe poses, decoder and compact voxel grads

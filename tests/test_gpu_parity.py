@@ -278,7 +278,7 @@ def test_prefilter_and_batch_max():
 
 
 # ------------------------------------------------------------------------------------ edge cases & properties
-@pytest.mark.parametrize("n_samples,n_surface,n_rays", [(5, 3, 37), (32, 16, 1), (16, 16, 333), (80, 16, 50), (32, 0, 64)])
+@pytest.mark.parametrize("n_samples,n_surface,n_rays", [(5, 3, 37), (4, 2, 29), (32, 16, 1), (16, 16, 333), (80, 16, 50), (32, 0, 64)])
 def test_ragged_shapes_against_oracle(n_samples, n_surface, n_rays):
     sc = su.load_scenes()["room0"]
     grids, dec_state = su.make_grids(sc, "soft"), su.load_decoders("soft")
