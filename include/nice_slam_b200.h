@@ -137,10 +137,13 @@ typedef struct {
                                     (N <= 256 rays, several decoders) one CTA per decoder and ray group.  Only the FP32-FMA back-end
                                     and the round-1 kernels accept NULL. */
   size_t split_workspace_bytes;
-  float* acts;                   /* optional [N,S,5,32] float32: outputs of the five hidden layers of the decoder whose WEIGHT gradients the
-                                    backward will be asked for (the colour decoder in stage color, src/Mapper.py:339-341).  When the forward
-                                    keeps them, the backward computes those weight gradients on the tensor cores (dW = dU^T X contracted over
-                                    the points of a tile) instead of the FP32-FMA pass that recomputes the forward.  NULL = not kept. */
+  float* acts;                   /* optional [n_kept][N,S,5,32] float32: outputs of the five hidden layers of the decoders whose WEIGHT
+                                    gradients the backward will be asked for (acts_levels).  When the forward keeps them, the backward computes
+                                    those weight gradients on the tensor cores (dW = dU^T X contracted over the points of a tile) instead of the
+                                    FP32-FMA pass that recomputes the forward.  NULL = not kept. */
+  int acts_levels;               /* which decoders' layer outputs `acts` holds: bit (1 << NSB_FINE) and / or (1 << NSB_COLOR), decoders of the
+                                    stage only, one [N,S,5,32] block each in level order (fine first).  0 = the colour decoder in stage color,
+                                    nothing otherwise (src/Mapper.py:339-341 with fix_fine; fix_fine = False adds the fine decoder). */
 } nsb_forward_outputs;
 
 /* Bytes of nsb_forward_outputs.split_workspace for n_rays rays of n_samples_total samples; non-zero for every n_rays >= 1 (0 for
@@ -175,6 +178,7 @@ typedef struct {
   double* d_c2w;
   int* pose_counter;
   const float* acts;             /* nsb_forward_outputs.acts of the same forward, or NULL */
+  int acts_levels;               /* nsb_forward_outputs.acts_levels of the same forward (0: the colour decoder in stage color) */
   void* result_dst;              /* optional (needs pose_dirs): once d_c2w is written, the same last CTA copies result_bytes bytes from result_src */
   const void* result_src;        /* to result_dst -- e.g. the block [d_rays_o | d_rays_d | loss | d c2w] to the device view of pinned host memory   */
   size_t result_bytes;           /* (nsb_host_device_pointer): the iteration's read-back without a copy node.  Both pointers 16-byte aligned.        */
@@ -263,6 +267,16 @@ int nsb_adam_mapper_step(const nsb_adam_voxel_group* groups, int n_groups, int d
                          double beta1, double beta2, double eps, void* stream);
 int nsb_adam_decoder(int level, const nsb_decoder_params* params, const float* grad_flat, float* exp_avg, float* exp_avg_sq,
                      double lr, double beta1, double beta2, double eps, int step, void* stream);
+/* nsb_adam_mapper_step with up to two decoders (NSB_MAX_ADAM_DECODERS), each with its own flat gradient, Adam state, learning rate and step
+ * count: with fix_fine = False the fine and colour decoders share the reference's parameter group 0 (Mapper.py:336-341, :368), but torch's
+ * Adam skips a parameter whose .grad is None, so each decoder's state advances only in the stages that evaluate it.  `params` is read
+ * during the call only.  n_decoders = 0 is an optimiser step over voxels alone. */
+#define NSB_MAX_ADAM_DECODERS 2
+typedef struct nsb_adam_decoder_item {
+  int level; const nsb_decoder_params* params; const float* grad_flat; float* exp_avg; float* exp_avg_sq; double lr; int step;
+} nsb_adam_decoder_item;
+int nsb_adam_mapper_step_decoders(const nsb_adam_voxel_group* groups, int n_groups, const nsb_adam_decoder_item* decoders, int n_decoders,
+                                  double beta1, double beta2, double eps, void* stream);
 
 /* Frustum feature selection (Mapper.get_mask_from_c2w, src/Mapper.py:93-164) of one grid, on the device: every voxel centre is
  * projected into the current frame (float32 camera transform, float64 intrinsics, like the reference's numpy code), the sensor
@@ -369,7 +383,8 @@ typedef struct {
   float* depth_max;                              /* [2]               batch depth maxima          */
   void* workspace; size_t workspace_bytes;       /* >= nsb_iteration_workspace_bytes(N)           */
   void* event_bwd_begin; void* event_bwd_end;    /* optional cudaEvent_t recorded around the backward launch (profiling hook) */
-  float* acts;                                   /* [N,S,5,32] or NULL (see nsb_forward_outputs.acts): needed for tensor-core weight gradients */
+  float* acts;                                   /* [n_kept][N,S,5,32] or NULL (see nsb_forward_outputs.acts): tensor-core weight gradients */
+  int acts_levels;                               /* see nsb_forward_outputs.acts_levels (0: the colour decoder in stage color) */
 } nsb_iteration_buffers;
 
 /* The workspace must be ZEROED ONCE after allocation (it contains the split_workspace counters, see nsb_forward_outputs). */

@@ -31,6 +31,11 @@ class DecoderParams(C.Structure):
                 ("Wc", C.c_void_p * 5), ("bc", C.c_void_p * 5), ("Wo", C.c_void_p), ("bo", C.c_void_p)]
 
 
+class AdamDecoderItem(C.Structure):
+    _fields_ = [("level", C.c_int), ("params", C.POINTER(DecoderParams)), ("grad_flat", C.c_void_p), ("exp_avg", C.c_void_p),
+                ("exp_avg_sq", C.c_void_p), ("lr", C.c_double), ("step", C.c_int)]
+
+
 class RenderInputs(C.Structure):
     _fields_ = [("stage", C.c_int32), ("n_rays", C.c_int32), ("n_samples", C.c_int32), ("n_surface", C.c_int32),
                 ("bound", C.c_double * 6), ("coarse_bound", C.c_double * 6),
@@ -42,7 +47,7 @@ class RenderInputs(C.Structure):
 class ForwardOutputs(C.Structure):
     _fields_ = [("depth", C.c_void_p), ("var", C.c_void_p), ("rgb", C.c_void_p),
                 ("z_vals", C.c_void_p), ("raw", C.c_void_p), ("corner_idx", C.c_void_p), ("masks", C.c_void_p),
-                ("split_workspace", C.c_void_p), ("split_workspace_bytes", C.c_size_t), ("acts", C.c_void_p)]
+                ("split_workspace", C.c_void_p), ("split_workspace_bytes", C.c_size_t), ("acts", C.c_void_p), ("acts_levels", C.c_int)]
 
 
 class BackwardArgs(C.Structure):
@@ -50,7 +55,7 @@ class BackwardArgs(C.Structure):
                 ("g_rgb", C.c_void_p), ("d_rays_o", C.c_void_p), ("d_rays_d", C.c_void_p),
                 ("d_grid", C.c_void_p * 4), ("d_flat", C.c_void_p * 4), ("workspace", C.c_void_p), ("masks", C.c_void_p),
                 ("slot_map", C.c_void_p * 4), ("split_workspace", C.c_void_p), ("split_workspace_bytes", C.c_size_t),
-                ("pose_dirs", C.c_void_p), ("d_c2w", C.c_void_p), ("pose_counter", C.c_void_p), ("acts", C.c_void_p),
+                ("pose_dirs", C.c_void_p), ("d_c2w", C.c_void_p), ("pose_counter", C.c_void_p), ("acts", C.c_void_p), ("acts_levels", C.c_int),
                 ("result_dst", C.c_void_p), ("result_src", C.c_void_p), ("result_bytes", C.c_size_t)]
 
 
@@ -62,7 +67,7 @@ class IterationBuffers(C.Structure):
     _fields_ = [("depth", C.c_void_p), ("var", C.c_void_p), ("rgb", C.c_void_p), ("z_vals", C.c_void_p), ("raw", C.c_void_p),
                 ("masks", C.c_void_p), ("g_depth", C.c_void_p), ("g_rgb", C.c_void_p), ("loss", C.c_void_p), ("depth_max", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
-                ("event_bwd_begin", C.c_void_p), ("event_bwd_end", C.c_void_p), ("acts", C.c_void_p)]
+                ("event_bwd_begin", C.c_void_p), ("event_bwd_end", C.c_void_p), ("acts", C.c_void_p), ("acts_levels", C.c_int)]
 
 
 class Peers(C.Structure):
@@ -111,6 +116,8 @@ SYMBOLS = {
     "nsb_adam_masked_voxels": (C.c_int, [C.POINTER(Grid), _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _P]),
     "nsb_adam_mapper_step": (C.c_int, [C.POINTER(AdamVoxelGroup), C.c_int, C.c_int, C.POINTER(DecoderParams), _P, _P, _P, C.c_double, C.c_int,
                                        C.c_double, C.c_double, C.c_double, _P]),
+    "nsb_adam_mapper_step_decoders": (C.c_int, [C.POINTER(AdamVoxelGroup), C.c_int, C.POINTER(AdamDecoderItem), C.c_int,
+                                                C.c_double, C.c_double, C.c_double, _P]),
     "nsb_adam_decoder": (C.c_int, [C.c_int, C.POINTER(DecoderParams), _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _P]),
     "nsb_frustum_mask_workspace": (C.c_size_t, [C.c_longlong]),
     "nsb_frustum_mask": (C.c_int, [C.POINTER(C.c_float), _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int,

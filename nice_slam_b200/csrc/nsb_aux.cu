@@ -503,21 +503,23 @@ __global__ void adam_flat_kernel(const AdamTable T, const float* __restrict__ gr
     }
 }
 
-// the mapper's whole optimiser step in ONE launch: CTAs [blk0[g], blk0[g+1]) update voxel group g, the last 32 CTAs the decoder
+// the mapper's whole optimiser step in ONE launch: CTAs [blk0[g], blk0[g+1]) update voxel group g, then dec_blocks CTAs per decoder
 struct MapperAdamArgs {
   nsb_grid g[4]; const int32_t* slots[4]; const float* grad[4]; float* em[4]; float* ev[4]; AdamScalars a[4]; int blk0[5]; int n_groups;
-  AdamTable T; const float* dgrad; float* dem; float* dev; AdamScalars da; int dec_blocks;
+  AdamTable T[NSB_MAX_ADAM_DECODERS]; const float* dgrad[NSB_MAX_ADAM_DECODERS]; float* dem[NSB_MAX_ADAM_DECODERS]; float* dev[NSB_MAX_ADAM_DECODERS];
+  AdamScalars da[NSB_MAX_ADAM_DECODERS]; int n_dec, dec_blocks;
 };
 __global__ void adam_mapper_kernel(const __grid_constant__ MapperAdamArgs A) {
   const int b = blockIdx.x;
-  if (b >= A.blk0[A.n_groups]) {                                   // decoder (adam_flat_kernel)
-    const int bd = b - A.blk0[A.n_groups];
-    for (int t = 0; t < A.T.count; t++)
-      for (int i = bd * blockDim.x + threadIdx.x; i < A.T.n[t]; i += A.dec_blocks * blockDim.x) {
-        const int f = A.T.off[t] + i;
-        float m = A.dem[f], v = A.dev[f];
-        A.T.param[t][i] = adam_update(A.T.param[t][i], A.dgrad[f], m, v, A.da);
-        A.dem[f] = m; A.dev[f] = v;
+  if (b >= A.blk0[A.n_groups]) {                                   // decoder k (adam_flat_kernel)
+    const int k = (b - A.blk0[A.n_groups]) / A.dec_blocks, bd = b - A.blk0[A.n_groups] - k * A.dec_blocks;
+    const AdamTable& T = A.T[k];
+    for (int t = 0; t < T.count; t++)
+      for (int i = bd * blockDim.x + threadIdx.x; i < T.n[t]; i += A.dec_blocks * blockDim.x) {
+        const int f = T.off[t] + i;
+        float m = A.dem[k][f], v = A.dev[k][f];
+        T.param[t][i] = adam_update(T.param[t][i], A.dgrad[k][f], m, v, A.da[k]);
+        A.dem[k][f] = m; A.dev[k][f] = v;
       }
     return;
   }
@@ -694,7 +696,14 @@ extern "C" int nsb_adam_decoder(int level, const nsb_decoder_params* p, const fl
 extern "C" int nsb_adam_mapper_step(const nsb_adam_voxel_group* groups, int n_groups, int dec_level, const nsb_decoder_params* dec_params,
                                     const float* dec_grad_flat, float* dec_exp_avg, float* dec_exp_avg_sq, double dec_lr, int dec_step,
                                     double beta1, double beta2, double eps, void* stream) {
+  nsb_adam_decoder_item d = {dec_level, dec_params, dec_grad_flat, dec_exp_avg, dec_exp_avg_sq, dec_lr, dec_step};
+  return nsb_adam_mapper_step_decoders(groups, n_groups, &d, dec_level >= 0 ? 1 : 0, beta1, beta2, eps, stream);
+}
+extern "C" int nsb_adam_mapper_step_decoders(const nsb_adam_voxel_group* groups, int n_groups, const nsb_adam_decoder_item* decoders, int n_decoders,
+                                             double beta1, double beta2, double eps, void* stream) {
   if (n_groups < 0 || n_groups > 4 || (n_groups > 0 && !groups)) { set_error("adam_mapper_step: 0..4 voxel groups"); return NSB_ERR_ARG; }
+  if (n_decoders < 0 || n_decoders > NSB_MAX_ADAM_DECODERS || (n_decoders > 0 && !decoders)) {
+    set_error("adam_mapper_step: 0..%d decoders", NSB_MAX_ADAM_DECODERS); return NSB_ERR_ARG; }
   MapperAdamArgs A; memset(&A, 0, sizeof(A));
   A.n_groups = n_groups;
   int rc;
@@ -707,13 +716,17 @@ extern "C" int nsb_adam_mapper_step(const nsb_adam_voxel_group* groups, int n_gr
     const long long n = (long long)G.grid.D * G.grid.H * G.grid.W;
     A.blk0[q + 1] = A.blk0[q] + (int)((n + 7) / 8 < 148 * 8 ? (n + 7) / 8 : 148 * 8);
   }
-  if (dec_level >= 0) {
-    if (dec_level > 3 || !dec_params || !dec_grad_flat || !dec_exp_avg || !dec_exp_avg_sq) { set_error("adam_mapper_step: bad decoder arguments"); return NSB_ERR_ARG; }
-    if ((rc = adam_scalars(dec_lr, beta1, beta2, eps, dec_step, &A.da))) return rc;
-    if ((rc = adam_table(dec_level, dec_params, &A.T))) return rc;
-    A.dgrad = dec_grad_flat; A.dem = dec_exp_avg; A.dev = dec_exp_avg_sq; A.dec_blocks = 32;
+  for (int k = 0; k < n_decoders; k++) {
+    const nsb_adam_decoder_item& D = decoders[k];
+    if (D.level < 0 || D.level > 3 || !D.params || !D.grad_flat || !D.exp_avg || !D.exp_avg_sq) { set_error("adam_mapper_step: bad decoder arguments"); return NSB_ERR_ARG; }
+    for (int j = 0; j < k; j++)
+      if (D.level == decoders[j].level) { set_error("adam_mapper_step: decoder %d given twice", D.level); return NSB_ERR_ARG; }
+    if ((rc = adam_scalars(D.lr, beta1, beta2, eps, D.step, &A.da[k]))) return rc;
+    if ((rc = adam_table(D.level, D.params, &A.T[k]))) return rc;
+    A.dgrad[k] = D.grad_flat; A.dem[k] = D.exp_avg; A.dev[k] = D.exp_avg_sq;
   }
-  const int blocks = A.blk0[n_groups] + A.dec_blocks;
+  A.n_dec = n_decoders; A.dec_blocks = 32;
+  const int blocks = A.blk0[n_groups] + A.n_dec * A.dec_blocks;
   if (blocks == 0) return NSB_OK;
   adam_mapper_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(A);
   return check_cuda(cudaGetLastError(), "adam_mapper_step launch");

@@ -37,7 +37,7 @@ static int forward_part(const nsb_render_inputs* in, const nsb_iteration_buffers
       in2->depth_max = b->depth_max;
     }
   }
-  nsb_forward_outputs fo = {b->depth, b->var, b->rgb, b->z_vals, b->raw, nullptr, b->masks, split_ptr(b, in->n_rays), split_room(b, in->n_rays), b->acts};
+  nsb_forward_outputs fo = {b->depth, b->var, b->rgb, b->z_vals, b->raw, nullptr, b->masks, split_ptr(b, in->n_rays), split_room(b, in->n_rays), b->acts, b->acts_levels};
   return render_forward_fused(in2, &fo, fs, stream);
 }
 
@@ -56,7 +56,7 @@ static FusedSeeds fused_seeds(const nsb_iteration_buffers* b, int kind, const vo
 static int backward_part(const nsb_render_inputs* in2, const nsb_iteration_buffers* b, const nsb_backward_args* g, void* stream, const PeerTail* tail = nullptr,
                          bool after_forward = false) {
   nsb_backward_args bw = *g;
-  bw.z_vals = b->z_vals; bw.raw = b->raw; bw.g_depth = b->g_depth; bw.g_var = nullptr; bw.g_rgb = b->g_rgb; bw.masks = b->masks; bw.acts = b->acts;
+  bw.z_vals = b->z_vals; bw.raw = b->raw; bw.g_depth = b->g_depth; bw.g_var = nullptr; bw.g_rgb = b->g_rgb; bw.masks = b->masks; bw.acts = b->acts; bw.acts_levels = b->acts_levels;
   bw.workspace = reinterpret_cast<char*>(b->workspace) + 16 + align16(nsb_tracking_seeds_workspace(in2->n_rays));
   bw.split_workspace = split_ptr(b, in2->n_rays); bw.split_workspace_bytes = split_room(b, in2->n_rays);
   if (b->event_bwd_begin) cudaEventRecord((cudaEvent_t)b->event_bwd_begin, (cudaStream_t)stream);

@@ -166,7 +166,7 @@ struct KParams {
   int tile_rays;                // backward: rays one tile can touch (stride of ray_parts per item)
   FusedSeeds fs;                // forward: loss seeds computed by the last CTA to finish (kind 0 = not fused)
   PeerTail tail;                // backward: sum of [loss | d c2w] over ranks by the last CTA (px.world <= 1: none)
-  int acts_lv;                  // forward: decoder level whose layer outputs go to fo.acts (-1: none)
+  int acts_mask;                // levels whose layer outputs fo.acts / bw.acts hold, one [N*S][5][32] block each in level order (acts_slot)
   int wbytes;                   // bytes reserved for the weight image in shared memory
   int max_pts, max_rays;        // per-CTA capacities the shared-memory carve-up was sized for
   nsb_sampling smp;             // lindisp / perturb uniforms / a given sorted z list (all zero: the default sampler)
@@ -1083,6 +1083,16 @@ static int weight_bytes(const int* dec, int n) {
   return wb;
 }
 
+// nsb_forward_outputs / nsb_backward_args .acts_levels -> K.acts_mask (0 keeps fill_common's default): the fine and colour decoders of the stage
+static int apply_acts_levels(KParams& K, int levels) {
+  if (levels == 0) return NSB_OK;
+  int stage_mask = 0; for (int i = 0; i < K.n_dec; i++) stage_mask |= 1 << K.dec[i];
+  if ((levels & ~((1 << NSB_FINE) | (1 << NSB_COLOR))) || (levels & ~stage_mask)) {
+    set_error("acts_levels 0x%x: only the fine / colour decoders of the stage keep layer outputs", levels); return NSB_ERR_ARG; }
+  K.acts_mask = levels;
+  return NSB_OK;
+}
+
 static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.in = *in;
   K.has_gt = (in->gt_depth != nullptr && in->stage != NSB_STAGE_COARSE) ? 1 : 0;    // Renderer.py:88-92
@@ -1094,7 +1104,7 @@ static void fill_common(KParams& K, const nsb_render_inputs* in) {
   memset(&K.fs, 0, sizeof(K.fs)); memset(&K.tail, 0, sizeof(K.tail));
   K.wbytes = weight_bytes(K.dec, K.n_dec);
   K.points = nullptr; K.points_raw = nullptr; K.n_points = 0;
-  K.acts_lv = in->stage == NSB_STAGE_COLOR ? 3 : -1;      // the colour decoder is the only one whose weights the mapper optimises (Mapper.py:339-341)
+  K.acts_mask = in->stage == NSB_STAGE_COLOR ? 1 << NSB_COLOR : 0;      // acts_levels = 0: the colour decoder (Mapper.py:339-341, fix_fine)
   memset(&K.smp, 0, sizeof(K.smp));
   for (int l = 0; l < 4; l++) K.d_packed[l] = nullptr;
 }
@@ -1348,6 +1358,7 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
   if (in->n_rays == 0) return NSB_OK;
   KParams K; fill_common(K, in); K.fo = *out; memset(&K.bw, 0, sizeof(K.bw));
   if ((rc = apply_sampling(K, smp))) return rc;
+  if ((rc = apply_acts_levels(K, out->acts_levels))) return rc;
   if (fs != nullptr) K.fs = *fs;
   const Family fam = kernel_family(K.S, in->n_rays, false);
   if (fam == Family::Fma) K.fo.masks = nullptr;                   // only the tensor-core forwards produce masks
@@ -1413,6 +1424,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   if (in->n_rays == 0) return NSB_OK;
   KParams K; fill_common(K, in); K.bw = *bw; memset(&K.fo, 0, sizeof(K.fo));
   if ((rc = apply_sampling(K, smp))) return rc;
+  if ((rc = apply_acts_levels(K, bw->acts_levels))) return rc;
   if (K.S > NSB_MAX_SAMPLES) { set_error("n_samples+n_surface = %d exceeds %d", K.S, NSB_MAX_SAMPLES); return NSB_ERR_UNSUPPORTED; }
   cudaStream_t st = (cudaStream_t)stream;
   bool any_w = false;
@@ -1448,9 +1460,9 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   int warps; size_t smem;
   if ((rc = fma_config(K, true, &warps, &smem))) return rc;
   // Plan: with the saved ReLU masks a tensor-core launch for the decoders that only need input gradients (rays, voxels), then one for those
-  // whose WEIGHT gradients are requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341): on the tensor cores when the
-  // forward kept its layer outputs (acts; one item per tile, one CTA per SM), else FP32-FMA, which recomputes the forward.  Without masks,
-  // or on the FP32-FMA back-end, one FP32-FMA launch for every decoder.
+  // whose WEIGHT gradients are requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341; with fix_fine = False also the
+  // fine decoder): on the tensor cores when they are fine / colour decoders whose layer outputs the forward kept (acts; one CTA per SM), else
+  // FP32-FMA, which recomputes the forward.  Without masks, or on the FP32-FMA back-end, one FP32-FMA launch for every decoder.
   enum Kind { TileIg, GroupIg, WgTile, Fma };
   const Family fam = kernel_family(K.S, in->n_rays, false);
   const bool sharded = tail != nullptr && tail->px.world > 1;
@@ -1464,7 +1476,8 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
       P.dec[P.n_dec] = K.dec[i]; P.dec_pos[P.n_dec] = i; P.n_dec++;
     }
     if (ig.n_dec > 0) { L[n] = ig; kind[n++] = fam == Family::Tile ? TileIg : GroupIg; }
-    const bool wg_tc = wg.n_dec == 1 && wg.dec[0] == NSB_COLOR && bw->acts != nullptr && fam == Family::Tile && g_wgrad_tc && !sharded;
+    bool wg_tc = wg.n_dec > 0 && bw->acts != nullptr && fam == Family::Tile && g_wgrad_tc && !sharded;
+    for (int i = 0; i < wg.n_dec; i++) wg_tc = wg_tc && (wg.dec[i] == NSB_FINE || wg.dec[i] == NSB_COLOR) && ((K.acts_mask >> wg.dec[i]) & 1);
     if (wg.n_dec > 0) { L[n] = wg; kind[n++] = wg_tc ? WgTile : Fma; }       // (every decoder here: wg == K)
   }
   // Every launch after the first adds to the ray gradients; the last one writes d c2w from its last CTA (the FP32-FMA kernel does not:
@@ -1482,7 +1495,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     else if (kind[i] == Fma) rc = launch_fma(P, true, st);
     else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true))) return rc;
     else if (kind[i] == WgTile) {
-      render_bwd_wg_tile_kernel<<<tiles, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
+      render_bwd_wg_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
       rc = check_cuda(cudaGetLastError(), "render_bwd_wg_tile_kernel launch");
     } else if (after_forward && !any_w && g_pdl) {
       // Programmatic dependent launch: the forward kernel signals `launch_dependents` when it starts, so this grid's CTAs become resident as

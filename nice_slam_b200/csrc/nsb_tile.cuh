@@ -616,7 +616,8 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
   NSB_PH(12);
 }
 
-// ---- tensor-core weight gradients (the colour decoder in the mapper's colour stage, src/Mapper.py:339-341,503) --------------------------------
+// ---- tensor-core weight gradients (the colour decoder in the mapper's colour stage, src/Mapper.py:339-341,503, and the fine decoder with -----
+// fix_fine = False) ---------------------------------------------------------------------------------------------------------------------
 // dW_i = DU_i^T X_i, dWc_i = G_i^T C, dWo = g_out^T H_4, dB = P^T DX are contractions over the POINTS of a tile: both operands of the MMA have the
 // points as K.  wgmma takes tf32 operands K-major only, so the epilogue threads write the rows they own a second time, transposed, into
 // [feature][point] tiles (the canonical no-swizzle layout with K = 128 points): DU_i and G_i form the A operand (M = 64 = [DU | G], hi tiles
@@ -627,6 +628,16 @@ constexpr int kMnTile = TM * 32;                               // floats of one 
 constexpr size_t kWgBytes = (size_t)6 * kMnTile * 4;           // A: DU hi, G hi, DU lo, G lo (64 KB)  B: one tile hi|lo (32 KB)
 constexpr int kWgALo = 2 * kMnTile, kWgBLo = kMnTile;          // offsets of the lo tiles
 struct WgSmem { float* du; float* g; float* b; float* dpk; };
+// block of decoder lv in fo.acts / bw.acts (levels of `mask` in level order), -1 if its layer outputs are not kept
+__host__ __device__ __forceinline__ int acts_slot(int mask, int lv) { return (mask >> lv) & 1 ? __builtin_popcount(mask & ((1 << lv) - 1)) : -1; }
+// packed-gradient offsets of the two weight-gradient decoders: fine (fc_c input [c_fine | c_middle], 64 wide; one output) and colour (32; four)
+struct WgDec { int o_W0, o_W1, o_W2, o_W3E, o_W3H, o_W4, o_WC, PC, o_WO, no, o_b, o_bc, o_bo; };
+template <int LV>
+__device__ __forceinline__ WgDec wg_dec() {
+  using D = Dec<LV>;
+  return WgDec{D::o_W0, D::o_W1, D::o_W2, D::o_W3E, D::o_W3H, D::o_W4, D::o_WC, D::PC, D::o_WO, D::NO, D::o_b, D::o_bc, D::o_bo};
+}
+static_assert(Dec<2>::PH == Dec<3>::PH && Dec<2>::PF == Dec<3>::PF && Dec<2>::o_B == Dec<3>::o_B, "shared pitches of the WG decoders");
 __device__ __forceinline__ void split4(const float4 v, float4& h, float4& l) {
   h = make_float4(tc::to_tf32(v.x), tc::to_tf32(v.y), tc::to_tf32(v.z), tc::to_tf32(v.w));
   l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
@@ -830,8 +841,9 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
   const int lane = threadIdx.x & 31, q = lane & 3;
   const int r0 = 64 * (threadIdx.x >> 7) + 16 * (warp & 3) + (lane >> 2);      // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8
   const int S = P.S;
-  using DW = Dec<3>;                                             // packed gradient image of the colour decoder (the only WG decoder)
-  float creg[kCW];                                               // WG: this thread's 16 grid features of its point
+  constexpr int PH = Dec<3>::PH, PF = Dec<3>::PF;                 // (the same for both WG decoders)
+  const WgDec DW = lv == 2 ? wg_dec<2>() : wg_dec<3>();          // packed gradient image of this WG decoder
+  float creg[kCW], cmid[kCW];                                    // WG: this thread's 16 grid features of its point (fine: + the middle grid's)
   const bool xyz = lv != 0;
   const float* hdr = t.hdr + hb * kHdrFloats;
   // ReLU bits of this thread's elements: word i of a row shifted right by 2 q puts column 8 j + 2 q + k on bit 8 j + k; row r0 + 8 goes to bits
@@ -867,6 +879,12 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
     __syncthreads();
     get_kt16(w->b, kWgBLo, row, cg, creg);
     __syncthreads();
+    if (lv == 2) {                                               // the fine decoder's fc_c also reads the middle features (no gradient into them)
+      gather_tile_kt(P.in.grid[NSB_MIDDLE], w->b, kWgBLo, G.xn, warp, lane);
+      __syncthreads();
+      get_kt16(w->b, kWgBLo, row, cg, cmid);
+      __syncthreads();
+    }
     // output layer: dWo = g_out^T H_4 (A block 0 = g_out in columns 0..3), dbo = column sums of g_out
     float go[kCW];
 #pragma unroll
@@ -879,11 +897,11 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       h4[4 * k] = v.x; h4[4 * k + 1] = v.y; h4[4 * k + 2] = v.z; h4[4 * k + 3] = v.w;
     }
     put_kt16(w->b, kWgBLo, row, cg, h4);
-    wg_group(*w, 0, w->dpk + DW::o_WO, DW::PH, 4);
+    wg_group(*w, 0, w->dpk + DW.o_WO, PH, DW.no);
     if (cg == 0) {
       const float sb = warp_colsum16(go, lane);
       const int col = colsum_col(lane);
-      if ((lane & 1) == 0 && col < 4) atomicAdd(w->dpk + DW::o_bo + col, sb);
+      if ((lane & 1) == 0 && col < DW.no) atomicAdd(w->dpk + DW.o_bo + col, sb);
     }
   }
 #pragma unroll 1
@@ -907,7 +925,7 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       }
       const float sb = frag_colsum(du, lane), sc = frag_colsum(d1, lane);
       const int col = frag_colsum_col(lane);
-      atomicAdd(w->dpk + DW::o_b + 32 * i + col, sb); atomicAdd(w->dpk + DW::o_bc + 32 * i + col, sc);
+      atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb); atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
     }
     fence_proxy_async();
     wg_bar_sync();                                               // this warpgroup's rows of G / DU are written -> its MMAs
@@ -924,11 +942,15 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
           xr[4 * k] = v.x; xr[4 * k + 1] = v.y; xr[4 * k + 2] = v.z; xr[4 * k + 3] = v.w;
         }
         put_kt16(w->b, kWgBLo, row, cg, xr);
-        const int o_wh = i == 1 ? DW::o_W1 : i == 2 ? DW::o_W2 : i == 3 ? DW::o_W3H : DW::o_W4;
-        wg_group(*w, 0, w->dpk + o_wh, DW::PH, 32);
+        const int o_wh = i == 1 ? DW.o_W1 : i == 2 ? DW.o_W2 : i == 3 ? DW.o_W3H : DW.o_W4;
+        wg_group(*w, 0, w->dpk + o_wh, PH, 32);
       }
       put_kt16(w->b, kWgBLo, row, cg, creg);                             // dWc_i = G_i^T C
-      wg_group(*w, 1, w->dpk + DW::o_WC + 32 * i * DW::PC, DW::PC, 32);
+      wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC, DW.PC, 32);
+      if (lv == 2) {                                             // fine: columns 32..63 of dWc_i = G_i^T C_middle (a second pass over the B tile)
+        put_kt16(w->b, kWgBLo, row, cg, cmid);
+        wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC + 32, DW.PC, 32);
+      }
       if (i == 3 || i == 0) {                                    // embedding part of W_0 / W_3
         const float* B = hdr + 464;
         for (int blk = 0; blk < 3; blk++) {
@@ -940,7 +962,7 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
             e[j] = f < kEmb ? __sinf(reduce_2pi(x)) : 0.0f;
           }
           put_kt16(w->b, kWgBLo, row, cg, e);
-          wg_group(*w, 0, w->dpk + (i == 0 ? DW::o_W0 : DW::o_W3E) + 32 * blk, DW::PF, 32);
+          wg_group(*w, 0, w->dpk + (i == 0 ? DW.o_W0 : DW.o_W3E) + 32 * blk, PF, 32);
         }
       }
       NSB_PH(24);
@@ -995,7 +1017,7 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       }
       if constexpr (WG) {                                        // dB[a][f] = sum_p p_a cos(.) dE_f  (embedder._B is a parameter of the decoder)
         const int nf = kEmb - 32 * c < 32 ? kEmb - 32 * c : 32;
-        wg_group(*w, 0, w->dpk + DW::o_B + 32 * c, kEmbPad, nf, true);
+        wg_group(*w, 0, w->dpk + Dec<3>::o_B + 32 * c, kEmbPad, nf, true);
       }
     }
   }
@@ -1169,7 +1191,8 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
       uint32_t* gm = P.fo.masks != nullptr ? P.fo.masks + (gp0 * 15 + qd * 5) : nullptr;
       const int dq = qd - q0;
       if (tid == 0 && qd + 1 < q1) load_header(P, t, P.dec[qd + 1], (dq + 1) & 1);      // (decoder qd-1 ended with CTA barriers: its buffer is free)
-      float* acts = (P.fo.acts != nullptr && lv == P.acts_lv) ? P.fo.acts + gp0 * 5 * 32 : nullptr;
+      const int as = acts_slot(P.acts_mask, lv);
+      float* acts = (P.fo.acts != nullptr && as >= 0) ? P.fo.acts + (as * NP + gp0) * 5 * 32 : nullptr;
       epi_forward<H16>(P, t, I, lv, G, n, dq & 1, (dq >> 1) & 1u, out, gm, acts, npts);
       if (lv == 3) { c0 = out[0]; c1 = out[1]; c2 = out[2]; } else occ += out[0];
       if (qd == 0 && cg == 0 && row < npts && P.fo.corner_idx != nullptr) {
@@ -1207,7 +1230,7 @@ __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_sampled_kerne
 // ================================================================================================================================
 // backward kernel (input gradients: rays + grid voxels)
 // ================================================================================================================================
-// WG = true: the item's decoder (the colour decoder) also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the
+// WG = true: the item's decoder (the colour or the fine decoder) also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the
 // "tensor-core weight gradients" helpers): 96 KB more shared memory in front of the common part -> one CTA per SM.
 template <bool WG>
 __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
@@ -1222,7 +1245,7 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   __shared__ int s_ndone, s_done[kMaxTileRays];
   WgSmem wg;
   wg.du = reinterpret_cast<float*>(sbase); wg.g = wg.du + kMnTile; wg.b = wg.du + 4 * kMnTile;
-  wg.dpk = WG ? P.d_packed[P.dec[0]] : nullptr;
+  wg.dpk = nullptr;
 
   const int nsplit = P.split;
   const int tile = blockIdx.x / nsplit, my = blockIdx.x - tile * nsplit;
@@ -1297,7 +1320,8 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
       const uint32_t* gm = P.bw.masks + (gp0 * 15 + P.dec_pos[qd] * 5);
       const int dq = qd - q0;
       if (tid == 0 && qd + 1 < q1) load_header(P, t, P.dec[qd + 1], (dq + 1) & 1);      // (the previous decoder ended with CTA barriers: its buffer is free)
-      const float* acts_row = (WG && row < npts) ? P.bw.acts + ((gp0 + row) * 5) * 32 + kCW * cg : nullptr;
+      if (WG) wg.dpk = P.d_packed[lv];
+      const float* acts_row = (WG && row < npts) ? P.bw.acts + ((acts_slot(P.acts_mask, lv) * NP + gp0 + row) * 5) * 32 + kCW * cg : nullptr;
       epi_backward<WG>(P, t, I, X, lv, G, dq & 1, (dq >> 1) & 1u, gm, npts, off0, gp0, WG ? &wg : nullptr, acts_row);
       epi_sync();                                                 // dL/dc rows + embedding partials visible
       const double* bb = lv == 0 ? P.in.coarse_bound : P.in.bound;

@@ -1,7 +1,7 @@
 """The joint-iteration loop of Mapper.optimize_map for NICE-SLAM (src/Mapper.py:296-379 set-up, :389-520 loop, :521-540 pose write-back),
-assembled from the library's pieces: frustum mask on the device -> voxel slot tables -> per iteration one fused mapping iteration
-(compact voxel gradients + colour-decoder gradients, steps.IterationContext) + fused Adam on the selected voxels (in place on the shared
-grids), on the colour decoder and -- with bundle adjustment -- on the camera tensors of the window (optim.FusedMapperAdam).
+assembled from the library's pieces: frustum mask on the device (or every voxel) -> voxel slot tables -> per iteration one fused mapping
+iteration (compact voxel gradients + the optimised decoders' gradients, steps.IterationContext) + fused Adam on the selected voxels (in place
+on the shared grids), on the optimised decoders and -- with bundle adjustment -- on the camera tensors of the window (optim.FusedMapperAdam).
 Pixel draws stay with the caller (the reference's get_sample_uv, torch RNG); with BA the rays are regenerated from the current camera
 tensors every iteration (nsb_window_rays), exactly as Mapper.py:437-462 does through get_camera_from_tensor + get_samples."""
 import ctypes as C
@@ -20,12 +20,20 @@ GRID_OF = {"middle": "grid_middle", "fine": "grid_fine", "color": "grid_color", 
 
 
 class FusedMappingLoop:
-    def __init__(self, renderer, c, decoders, c2w, depth, keys=("grid_middle", "grid_fine", "grid_color"), w_color=0.2, capacity=1024):
+    def __init__(self, renderer, c, decoders, c2w, depth, keys=("grid_middle", "grid_fine", "grid_color"), w_color=0.2, capacity=1024,
+                 fix_fine=True, fix_color=False, frustum_feature_selection=True):
         """c: the shared grids dict (updated in place); c2w / depth: pose and sensor depth of the current frame (frustum selection);
-        capacity: rays per iteration the buffers are sized for (cfg['mapping']['pixels'])."""
+        capacity: rays per iteration the buffers are sized for (cfg['mapping']['pixels']).  fix_fine / fix_color /
+        frustum_feature_selection: the mapper's settings of the same names (Mapper.py:296-345): a decoder that is not fixed is optimised
+        in the stages that evaluate it; without frustum feature selection every voxel of each grid is a parameter (c2w / depth unused).
+        The colour-refinement pass of the last frame (Mapper.py:578-586) is fix_color=True, frustum_feature_selection=False."""
         require_default_sampling(renderer, "FusedMappingLoop")
         self.r, self.c, self.dec, self.w_color, self.capacity = renderer, c, decoders, w_color, int(capacity)
-        self.masked = {k: MaskedVoxels(c[k], frustum_voxel_mask(renderer, c2w, k, c[k], depth)) for k in keys}
+        self.fix_fine, self.fix_color, self.frustum_feature_selection = bool(fix_fine), bool(fix_color), bool(frustum_feature_selection)
+        if frustum_feature_selection:
+            self.masked = {k: MaskedVoxels(c[k], frustum_voxel_mask(renderer, c2w, k, c[k], depth)) for k in keys}
+        else:                                                     # Mapper.py:302-312: the whole grid, through the same slot tables
+            self.masked = {k: MaskedVoxels(c[k], torch.ones(c[k].shape[2:], dtype=torch.bool, device=c[k].device)) for k in keys}
         self.adam = FusedMapperAdam()
         self._ctx = {}
         self.n_frames = 0
@@ -103,6 +111,11 @@ class FusedMappingLoop:
                                     self.adam.betas[0], self.adam.betas[1], self.adam.eps, b["step"], _stream()), "nsb_adam_poses")
         return loss
 
+    def grad_decoders(self, stage):
+        """The decoders whose parameters get a gradient at `stage`: those of parameter group 0 (the fine decoder unless fix_fine, the colour
+        decoder unless fix_color, Mapper.py:336-341) that the stage evaluates (decoder.py:317-342); torch's Adam skips the others."""
+        return tuple(lvl for lvl, fixed in (("fine", self.fix_fine), ("color", self.fix_color)) if not fixed and lvl in STAGE_DECODERS[stage])
+
     def _context(self, n, stage, device):
         """ONE context per stage, sized for a capacity: the ray count after the bbox pre-filter changes almost every iteration
         (Mapper.py:471-481) and must not allocate a fresh set of buffers each time.  The capacity grows geometrically if ever exceeded."""
@@ -111,7 +124,7 @@ class FusedMappingLoop:
             cap = max(n, self.capacity, 2 * ctx.n if ctx is not None else 0)
             grids = tuple(GRID_OF[l] for l in STAGE_DECODERS[stage] if GRID_OF[l] in self.masked)
             ctx = IterationContext(self.r, cap, stage, device, kind="map", grad_grids=grids,
-                                   grad_decoders=("color",) if stage == "color" else (), masked=self.masked, host_staging=False,
+                                   grad_decoders=self.grad_decoders(stage), masked=self.masked, host_staging=False,
                                    n_frames=self.n_frames)
             self._ctx[stage] = ctx
         return ctx
@@ -125,10 +138,11 @@ class FusedMappingLoop:
         return loss
 
     def _optimiser_step(self, ctx, stage, lr):
-        """optimizer.step() (Mapper.py:504) for the param groups whose parameters received a gradient (Adam skips the others): the selected
-        voxels of the stage's grids and, in stage 'color', the colour decoder -- one launch (optim.FusedMapperAdam.step_all)."""
+        """optimizer.step() (Mapper.py:504) for the parameters that received a gradient (Adam skips the others): the selected voxels of the
+        stage's grids and the stage's optimised decoders (grad_decoders), all at the decoders_lr of the stage -- one launch
+        (optim.FusedMapperAdam.step_all)."""
         vox = [(key, self.c[key], self.masked[key], ctx.d_grid[key], lr[key[5:]]) for key in ctx.grad_grids]
-        dec = ("color", self.dec, ctx.d_flat["color"], lr["decoders"]) if stage == "color" else None
+        dec = [(lvl, self.dec, ctx.d_flat[lvl], lr["decoders"]) for lvl in ctx.grad_decoders]
         self.adam.step_all(vox, dec, renderer=self.r)
 
 

@@ -38,12 +38,16 @@ class FusedMapperAdam:
                                                      _VP(st["v"].data_ptr()), float(lr), self.betas[0], self.betas[1], self.eps, st["step"], _stream()),
                    "nsb_adam_masked_voxels")
 
-    def step_all(self, voxel_items, decoder_item=None, renderer=None):
+    def step_all(self, voxel_items, decoder_items=(), renderer=None):
         """The mapper's whole optimizer.step() (Mapper.py:504) in ONE launch.  voxel_items: [(key, grid, masked, grad, lr)] (at most four, as
-        step_voxels); decoder_item: (level_name, decoders, grad_flat, lr) or None (as step_decoder)."""
+        step_voxels); decoder_items: [(level_name, decoders, grad_flat, lr)] (at most two, as step_decoder), the decoders that received a
+        gradient in this iteration: each keeps its own Adam state and step count, as torch.optim.Adam does for the parameters of one group
+        whose .grad is set.  Pass the FusedRenderer so that its packed-weight cache of every stepped decoder is invalidated."""
         items = [it for it in voxel_items if it[2].count > 0]
         if len(items) > 4:
             raise RuntimeError("nice_slam_b200: at most four voxel groups per fused optimiser step")
+        if len(decoder_items) > 2:
+            raise RuntimeError("nice_slam_b200: at most two decoders per fused optimiser step")
         groups = (_lib.AdamVoxelGroup * max(len(items), 1))()
         for q, (key, grid, masked, grad, lr) in enumerate(items):
             st = self._st(key, masked.count * 32, grid.device)
@@ -52,19 +56,17 @@ class FusedMapperAdam:
             g.grid = grid_struct(grid.detach())
             g.slot_map, g.grad, g.exp_avg, g.exp_avg_sq = masked.slot_map.data_ptr(), grad.data_ptr(), st["m"].data_ptr(), st["v"].data_ptr()
             g.lr, g.step = float(lr), st["step"]
-        li, dp, gf, dm, dv, dlr, dstep = -1, None, None, None, None, 0.0, 0
-        if decoder_item is not None:
-            level_name, decoders, grad_flat, dlr = decoder_item
-            li = LEVELS.index(level_name)
+        decs = (_lib.AdamDecoderItem * max(len(decoder_items), 1))()
+        for k, (level_name, decoders, grad_flat, lr) in enumerate(decoder_items):
             st = self._st("dec_" + level_name, grad_flat.numel(), grad_flat.device)
             st["step"] += 1
-            dstep = st["step"]
-            dp = C.byref(self._decoder_struct(decoders, level_name))
-            gf, dm, dv = _VP(grad_flat.data_ptr()), _VP(st["m"].data_ptr()), _VP(st["v"].data_ptr())
-        _lib.check(_lib.lib().nsb_adam_mapper_step(groups, len(items), li, dp, gf, dm, dv, float(dlr), dstep,
-                                                   self.betas[0], self.betas[1], self.eps, _stream()), "nsb_adam_mapper_step")
-        if decoder_item is not None and renderer is not None:
-            renderer.invalidate_decoders((decoder_item[0],))
+            d = decs[k]
+            d.level, d.params = LEVELS.index(level_name), C.pointer(self._decoder_struct(decoders, level_name))
+            d.grad_flat, d.exp_avg, d.exp_avg_sq, d.lr, d.step = grad_flat.data_ptr(), st["m"].data_ptr(), st["v"].data_ptr(), float(lr), st["step"]
+        _lib.check(_lib.lib().nsb_adam_mapper_step_decoders(groups, len(items), decs, len(decoder_items), self.betas[0], self.betas[1], self.eps,
+                                                            _stream()), "nsb_adam_mapper_step_decoders")
+        if decoder_items and renderer is not None:
+            renderer.invalidate_decoders(tuple(it[0] for it in decoder_items))
 
     def _decoder_struct(self, decoders, level_name):
         """nsb_decoder_params of a decoder, cached on the storage pointers of its parameters (building it walks ~20 tensors)."""

@@ -207,14 +207,16 @@ class _RenderFn(torch.autograd.Function):
         inp = _inputs(call, ro, rd, depth_max, t_u, t_s, data)
         masks = torch.empty(n, S, 15, dtype=torch.int32, device=dev)      # ReLU sign bits: lets backward skip the forward recompute
         out.masks = masks.data_ptr()
-        # colour-decoder parameters that need a gradient (the mapper's colour stage, Mapper.py:339-341): keep the decoder's layer outputs so that
-        # the backward computes the weight gradients on the tensor cores
-        acts = None
-        if call.stage == "color":
-            k0 = 3 + n_lvl + sum(len(call.param_names[l]) for l in call.levels[: call.levels.index("color")])
-            if any(ctx.needs_input_grad[k0 + i] for i in range(len(call.param_names["color"]))):
-                acts = torch.empty(n, S, 5, 32, dtype=torch.float32, device=dev)
-                out.acts = acts.data_ptr()
+        # decoders whose parameters need a gradient: when they are fine / colour decoders (the mapper's colour stage, Mapper.py:339-341, and the
+        # fine decoder with fix_fine = False) keep their layer outputs so that the backward computes the weight gradients on the tensor cores
+        k0, graded = 3 + n_lvl, []
+        for lvl in call.levels:
+            if any(ctx.needs_input_grad[k0 + i] for i in range(len(call.param_names[lvl]))):
+                graded.append(lvl)
+            k0 += len(call.param_names[lvl])
+        acts, acts_levels = acts_buffer(graded, call.levels, n, S, dev)
+        if acts is not None:
+            out.acts, out.acts_levels = acts.data_ptr(), acts_levels
         corner = None
         if call.aux is not None:
             corner = torch.empty(n, S, 3, dtype=torch.int32, device=dev)
@@ -226,7 +228,7 @@ class _RenderFn(torch.autograd.Function):
         ctx.call = call
         ctx.n_lvl = n_lvl
         ctx.keep = (ro, rd, depth_max, t_u, t_s, z_vals, raw, masks, split)
-        ctx.acts = acts
+        ctx.acts, ctx.acts_levels = acts, acts_levels
         ctx.grids = data
         ctx.param_shapes = [tuple(p.shape) for p in params]
         return depth, var, rgb
@@ -246,7 +248,7 @@ class _RenderFn(torch.autograd.Function):
         if split is not None:
             bw.split_workspace, bw.split_workspace_bytes = split.data_ptr(), split.numel()
         if ctx.acts is not None:
-            bw.acts = ctx.acts.data_ptr()
+            bw.acts, bw.acts_levels = ctx.acts.data_ptr(), ctx.acts_levels
         gd = g_depth.detach().contiguous().double() if g_depth is not None else torch.zeros(n, dtype=torch.float64, device=dev)
         gv = g_var.detach().contiguous().double() if g_var is not None else None
         gc = g_rgb.detach().contiguous().float() if g_rgb is not None else None
@@ -303,6 +305,15 @@ class _RenderFn(torch.autograd.Function):
             mv = call.masked[j]
             d_grids[j] = mv.to_reference(dg[: mv.count]) if mv.count > 0 else torch.zeros(0, dtype=torch.float32, device=dev)
         return (None, d_o if needs[1] else None, d_d if needs[2] else None, *d_grids, *d_params)
+
+
+def acts_buffer(grad_decoders, levels, n, S, device):
+    """(acts [k,n,S,5,32] float32 or None, acts_levels bit mask) for the stage decoders `levels` of which `grad_decoders` want weight gradients:
+    the tensor-core weight-gradient kernel serves a non-empty set of fine / colour decoders from their kept layer outputs."""
+    wg = [lvl for lvl in LEVELS if lvl in grad_decoders and lvl in levels]
+    if not wg or not set(wg) <= {"fine", "color"}:
+        return None, 0
+    return torch.empty(len(wg), n, S, 5, 32, dtype=torch.float32, device=device), sum(1 << LEVELS.index(lvl) for lvl in wg)
 
 
 def require_default_sampling(renderer, what):

@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import LEVELS, STAGE_DECODERS
-from .renderer import _VP, _inputs, _linspaces, _stream, _Call, _require_cuda, require_default_sampling
+from .renderer import _VP, _inputs, _linspaces, _stream, _Call, _require_cuda, acts_buffer, require_default_sampling
 
 KERNEL_LAUNCHES_PER_ITERATION = 2       # render_fwd + render_bwd for batches <= 1024 rays: the forward reduces the batch depth maxima itself and
                                         # its last CTA computes the loss seeds, the backward's last CTA produces d c2w; larger batches add
@@ -98,13 +98,14 @@ class IterationContext:
         self.d_frames = self.packed[4: 4 + 12 * self.n_frames].view(self.n_frames, 12)
         self.d_grid = {key: self.packed[sect[key][0]: sect[key][0] + sect[key][1]].view(-1, 32) for key in self.grad_grids if key in self.masked}
         self.d_flat = {lvl: self.packed[sect["dec_" + lvl][0]: sect["dec_" + lvl][0] + sect["dec_" + lvl][1]] for lvl in self.grad_decoders}
-        # layer outputs of the colour decoder, kept by the forward when its weight gradients are wanted: the backward then computes them on the
-        # tensor cores (nsb_forward_outputs.acts); 640 B per sample point
-        self.acts = torch.empty(n, S, 5, 32, dtype=f32, device=dev) if (stage == "color" and "color" in self.grad_decoders) else None
+        # layer outputs of the fine / colour decoders, kept by the forward when their weight gradients are wanted: the backward then computes them
+        # on the tensor cores (nsb_forward_outputs.acts / acts_levels); 640 B per sample point and decoder.  A set with the middle or coarse
+        # decoder takes the FP32-FMA pass, which reads no acts.
+        self.acts, self.acts_levels = acts_buffer(self.grad_decoders, self.levels, n, S, dev)
         self.buf = _lib.IterationBuffers(self.depth.data_ptr(), self.var.data_ptr(), self.rgb.data_ptr(), self.z_vals.data_ptr(),
                                          self.raw.data_ptr(), self.masks.data_ptr(), self.g_depth.data_ptr(), self.g_rgb.data_ptr(), self.loss.data_ptr(),
                                          self.depth_max.data_ptr(), self.ws.data_ptr(), self.ws.numel(), None, None,
-                                         self.acts.data_ptr() if self.acts is not None else None)
+                                         self.acts.data_ptr() if self.acts is not None else None, self.acts_levels)
         self.ev_bwd = None
         # pinned host staging for run_host(): [rays_o | rays_d | gt_depth] f32, gt_color, and the read-back block
         cuda = dev.type == "cuda" and host_staging      # (pin_memory is a synchronising cudaHostAlloc: skipped when run_host() is never used)
@@ -152,11 +153,11 @@ class IterationContext:
         acts = self.acts.data_ptr() if self.acts is not None else None
         split = self.split_ws.data_ptr() if self.split_bytes else None
         fo = _lib.ForwardOutputs(self.depth.data_ptr(), self.var.data_ptr(), self.rgb.data_ptr(), self.z_vals.data_ptr(), self.raw.data_ptr(), None,
-                                 self.masks.data_ptr(), split, self.split_bytes, acts)
+                                 self.masks.data_ptr(), split, self.split_bytes, acts, self.acts_levels)
         bw = self._grads(c)
         bw.z_vals, bw.raw, bw.g_depth, bw.g_rgb, bw.masks = (self.z_vals.data_ptr(), self.raw.data_ptr(), self.g_depth.data_ptr(),
                                                               self.g_rgb.data_ptr(), self.masks.data_ptr())
-        bw.split_workspace, bw.split_workspace_bytes, bw.acts = split, self.split_bytes, acts
+        bw.split_workspace, bw.split_workspace_bytes, bw.acts, bw.acts_levels = split, self.split_bytes, acts, self.acts_levels
         return call, grids, inp, fo, bw
 
     def zero_grads(self):
