@@ -3,6 +3,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 #include <cuda_fp16.h>
 #include "nsb_common.cuh"
 #include "nsb_seeds.cuh"
@@ -81,20 +82,21 @@ __global__ void pack_kernel(const __grid_constant__ PackArgs A) {
 }
 
 // ---- tensor-core operand images (layout: nsb_common.cuh) --------------------------------------------------------------------
-// hi | lo of a [R x 32] canonical tile whose element (row, k) is get(row, k)
+// hi | lo of a [R x KW] canonical tile ([row/8][k/4][row%8][k%4]) whose element (row, k) is get(row, k)
 template <typename F>
-__device__ __forceinline__ void emit_tile(float*& dst, int& e, int R, F&& get) {
-  float* hi = dst; float* lo = dst + R * 32;
-  dst += 2 * R * 32;
+__device__ __forceinline__ void emit_unit(float*& dst, int& e, int R, int KW, F&& get) {
+  float* hi = dst; float* lo = dst + R * KW;
+  dst += 2 * R * KW;
   if (!pk_mine(e)) return;
-  for (int idx = threadIdx.x; idx < R * 32; idx += blockDim.x) {
-    const int r = idx >> 5, k = idx & 31;
+  for (int idx = threadIdx.x; idx < R * KW; idx += blockDim.x) {
+    const int r = idx / KW, k = idx - r * KW;
     const float v = get(r, k);
     const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);          // the 19 bits the tensor core reads (nsb_tc.cuh)
-    const int o = ((r >> 3) * 8 + (k >> 2)) * 32 + (r & 7) * 4 + (k & 3);
+    const int o = ((r >> 3) * (KW >> 2) + (k >> 2)) * 32 + (r & 7) * 4 + (k & 3);
     hi[o] = h; lo[o] = v - h;
   }
 }
+// round-1 images: [R x 32] tiles
 template <int LV>
 __device__ void pack_operands_level(float* __restrict__ img /* packed image of this level: raw part already written */, int& e) {
   using D = Dec<LV>;
@@ -115,33 +117,19 @@ __device__ void pack_operands_level(float* __restrict__ img /* packed image of t
   dst += kHdrFloats;
   if (D::XYZ)
     for (int h = 0; h < D::CD / 32; h++)
-      emit_tile(dst, e, 160, [&](int r, int k) { return W[D::o_WC + r * D::PC + 32 * h + k]; });          // row r = 32 i + o
+      emit_unit(dst, e, 160, 32, [&](int r, int k) { return W[D::o_WC + r * D::PC + 32 * h + k]; });          // row r = 32 i + o
   for (int b = 0; b < op_nblk(LV); b++)
-    emit_tile(dst, e, 64, [&](int r, int k) { return W[(r < 32 ? D::o_W0 : D::o_W3E) + (r & 31) * D::PF + 32 * b + k]; });
-  for (int i = 1; i < 5; i++) emit_tile(dst, e, 32, [&](int r, int k) { return W[o_wh[i] + r * PH + k]; });
+    emit_unit(dst, e, 64, 32, [&](int r, int k) { return W[(r < 32 ? D::o_W0 : D::o_W3E) + (r & 31) * D::PF + 32 * b + k]; });
+  for (int i = 1; i < 5; i++) emit_unit(dst, e, 32, 32, [&](int r, int k) { return W[o_wh[i] + r * PH + k]; });
   // backward (transposed operands)
   dst = img + op_bwd_offset(LV);
   for (int i = 4; i >= 0; i--) {
-    if (D::XYZ) emit_tile(dst, e, D::CD, [&](int c, int k) { return W[D::o_WC + (i * 32 + k) * D::PC + c]; });
-    if (i >= 1) emit_tile(dst, e, 32, [&](int j, int k) { return W[o_wh[i] + k * PH + j]; });
-    if (i == 3 || i == 0) emit_tile(dst, e, D::FIRSTP, [&](int f, int k) { return W[(i == 0 ? D::o_W0 : D::o_W3E) + k * D::PF + f]; });
+    if (D::XYZ) emit_unit(dst, e, D::CD, 32, [&](int c, int k) { return W[D::o_WC + (i * 32 + k) * D::PC + c]; });
+    if (i >= 1) emit_unit(dst, e, 32, 32, [&](int j, int k) { return W[o_wh[i] + k * PH + j]; });
+    if (i == 3 || i == 0) emit_unit(dst, e, D::FIRSTP, 32, [&](int f, int k) { return W[(i == 0 ? D::o_W0 : D::o_W3E) + k * D::PF + f]; });
   }
 }
 // ---- v2 operand images: units for the tile kernels (layout: nsb_common.cuh op2_*) -------------------------------------------------
-// hi | lo of a [R x KW] canonical tile ([row/8][k/4][row%8][k%4]) whose element (row, k) is get(row, k)
-template <typename F>
-__device__ __forceinline__ void emit_unit(float*& dst, int& e, int R, int KW, F&& get) {
-  float* hi = dst; float* lo = dst + R * KW;
-  dst += 2 * R * KW;
-  if (!pk_mine(e)) return;
-  for (int idx = threadIdx.x; idx < R * KW; idx += blockDim.x) {
-    const int r = idx / KW, k = idx - r * KW;
-    const float v = get(r, k);
-    const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-    const int o = ((r >> 3) * (KW >> 2) + (k >> 2)) * 32 + (r & 7) * 4 + (k & 3);
-    hi[o] = h; lo[o] = v - h;
-  }
-}
 template <int LV>
 __device__ void pack_units_level(float* __restrict__ img, int& e) {
   using D = Dec<LV>;
@@ -280,33 +268,27 @@ __global__ void mapping_seeds_kernel(const double* __restrict__ depth, const flo
 }
 
 
-// d c2w from ray gradients (single CTA, deterministic)
-__global__ void pose_grad_kernel(const float* __restrict__ dirs, const float* __restrict__ dro, const float* __restrict__ drd, int n,
-                                 double* __restrict__ out, const double* __restrict__ loss_local, const PeerX px) {
+// d c2w from ray gradients, deterministic: CTA b sums rows [offs[b], offs[b + 1]) into out[12 b ...], or, with offs NULL, one CTA sums rows
+// [0, n) (double output only: with px.world > 1 summed over the ranks as well).
+template <typename T>
+__global__ void pose_grad_kernel(const float* __restrict__ dirs, const float* __restrict__ dro, const float* __restrict__ drd,
+                                 const int32_t* __restrict__ offs, int n, T* __restrict__ out, const double* __restrict__ loss_local, const PeerX px) {
   __shared__ double red[32];
   double acc[12];
-#pragma unroll
-  for (int k = 0; k < 12; k++) acc[k] = 0.0;
-  for (int r = threadIdx.x; r < n; r += blockDim.x) {
-#pragma unroll
-    for (int i = 0; i < 3; i++) {
-      const double g = (double)drd[3 * r + i];
-#pragma unroll
-      for (int j = 0; j < 3; j++) acc[4 * i + j] += g * (double)dirs[3 * r + j];
-      acc[4 * i + 3] += (double)dro[3 * r + i];
-    }
-  }
+  pose_grad_partial(dirs, dro, drd, offs ? offs[blockIdx.x] : 0, offs ? offs[blockIdx.x + 1] : n, acc);
   __shared__ double tot[13];
   for (int k = 0; k < 12; k++) { const double t = block_sum(acc[k], red); if (threadIdx.x == 0) tot[k + 1] = t; }
-  if (px.world <= 1) {
-    if (threadIdx.x == 0) for (int k = 0; k < 12; k++) out[k] = tot[k + 1];
-    return;
+  if constexpr (std::is_same_v<T, double>) {
+    if (px.world > 1) {
+      // SUM over ranks of [loss | d c2w] through peer memory (channel 2: slot = 13 doubles + flag in 128 bytes); out = 13 doubles.
+      __shared__ uint32_t s_seq;
+      if (threadIdx.x == 0) tot[0] = loss_local != nullptr ? loss_local[0] : 0.0;
+      __syncthreads();
+      peer_sum13(px, tot, 13, out, &s_seq);
+      return;
+    }
   }
-  // SUM over ranks of [loss | d c2w] through peer memory (channel 2: slot = 13 doubles + flag in 128 bytes); out = 13 doubles.
-  __shared__ uint32_t s_seq;
-  if (threadIdx.x == 0) tot[0] = loss_local != nullptr ? loss_local[0] : 0.0;
-  __syncthreads();
-  peer_sum13(px, tot, 13, out, &s_seq);
+  if (threadIdx.x == 0) for (int k = 0; k < 12; k++) out[12 * blockIdx.x + k] = (T)tot[k + 1];
 }
 
 // ---- masked voxel parameterisation (Mapper.py:317-333, :393-401, :511-519) --------------------------------------------
@@ -476,12 +458,13 @@ __device__ __forceinline__ float adam_update(float p, float g, float& m, float& 
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), a.inv_bc2_sqrt_div), a.eps);   // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
   return __fadd_rn(p, __fmul_rn(a.neg_step, __fdiv_rn(m, denom)));                     // param.addcdiv_(exp_avg, denom, value=-step_size)
 }
-// one warp per voxel, lane = channel: the parameters ARE the selected voxels of the shared grid (updated in place)
-__global__ void adam_masked_kernel(nsb_grid g, const int32_t* __restrict__ slots, const float* __restrict__ grad, float* __restrict__ em,
-                                   float* __restrict__ ev, const AdamScalars a) {
+// The element updates of one parameter group, spread over CTA cta of n_ctas (updates are element-wise: the split does not change a bit).
+// Voxel group: one warp per voxel, lane = channel; the parameters ARE the selected voxels of the shared grid (updated in place).
+__device__ __forceinline__ void adam_voxel_group(const nsb_grid& g, const int32_t* __restrict__ slots, const float* __restrict__ grad,
+                                                 float* __restrict__ em, float* __restrict__ ev, const AdamScalars& a, int cta, int n_ctas) {
   const long long n = (long long)g.D * g.H * g.W;
   const int lane = threadIdx.x & 31;
-  for (long long vx = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); vx < n; vx += (long long)gridDim.x * (blockDim.x >> 5)) {
+  for (long long vx = (long long)cta * (blockDim.x >> 5) + (threadIdx.x >> 5); vx < n; vx += (long long)n_ctas * (blockDim.x >> 5)) {
     const int s = __ldg(slots + vx);
     if (s < 0) continue;
     const int w = (int)(vx % g.W), h = (int)((vx / g.W) % g.H), d = (int)(vx / ((long long)g.W * g.H));
@@ -492,10 +475,12 @@ __global__ void adam_masked_kernel(nsb_grid g, const int32_t* __restrict__ slots
     em[i] = m; ev[i] = v;
   }
 }
+// Decoder: its parameter tensors, each at its offset in the flat gradient / state (canonical order, flat_offset).
 struct AdamTable { float* param[24]; int off[24]; int n[24]; int count; };
-__global__ void adam_flat_kernel(const AdamTable T, const float* __restrict__ grad, float* __restrict__ em, float* __restrict__ ev, const AdamScalars a) {
+__device__ __forceinline__ void adam_decoder_table(const AdamTable& T, const float* __restrict__ grad, float* __restrict__ em, float* __restrict__ ev,
+                                                   const AdamScalars& a, int cta, int n_ctas) {
   for (int t = 0; t < T.count; t++)
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < T.n[t]; i += gridDim.x * blockDim.x) {
+    for (int i = cta * blockDim.x + threadIdx.x; i < T.n[t]; i += n_ctas * blockDim.x) {
       const int f = T.off[t] + i;
       float m = em[f], v = ev[f];
       T.param[t][i] = adam_update(T.param[t][i], grad[f], m, v, a);
@@ -511,54 +496,14 @@ struct MapperAdamArgs {
 };
 __global__ void adam_mapper_kernel(const __grid_constant__ MapperAdamArgs A) {
   const int b = blockIdx.x;
-  if (b >= A.blk0[A.n_groups]) {                                   // decoder k (adam_flat_kernel)
+  if (b >= A.blk0[A.n_groups]) {
     const int k = (b - A.blk0[A.n_groups]) / A.dec_blocks, bd = b - A.blk0[A.n_groups] - k * A.dec_blocks;
-    const AdamTable& T = A.T[k];
-    for (int t = 0; t < T.count; t++)
-      for (int i = bd * blockDim.x + threadIdx.x; i < T.n[t]; i += A.dec_blocks * blockDim.x) {
-        const int f = T.off[t] + i;
-        float m = A.dem[k][f], v = A.dev[k][f];
-        T.param[t][i] = adam_update(T.param[t][i], A.dgrad[k][f], m, v, A.da[k]);
-        A.dem[k][f] = m; A.dev[k][f] = v;
-      }
+    adam_decoder_table(A.T[k], A.dgrad[k], A.dem[k], A.dev[k], A.da[k], bd, A.dec_blocks);
     return;
   }
   int q = 0;
   while (q + 1 < A.n_groups && b >= A.blk0[q + 1]) q++;
-  const nsb_grid& g = A.g[q];
-  const int nb = A.blk0[q + 1] - A.blk0[q], bq = b - A.blk0[q];
-  const long long n = (long long)g.D * g.H * g.W;
-  const int lane = threadIdx.x & 31;
-  for (long long vx = (long long)bq * (blockDim.x >> 5) + (threadIdx.x >> 5); vx < n; vx += (long long)nb * (blockDim.x >> 5)) {      // (adam_masked_kernel)
-    const int s = __ldg(A.slots[q] + vx);
-    if (s < 0) continue;
-    const int w = (int)(vx % g.W), h = (int)((vx / g.W) % g.H), d = (int)(vx / ((long long)g.W * g.H));
-    float* cell = const_cast<float*>(g.data) + d * g.stride_d + h * g.stride_h + w * g.stride_w + lane * g.stride_c;
-    const long long i = (long long)s * 32 + lane;
-    float m = A.em[q][i], v = A.ev[q][i];
-    *cell = adam_update(*cell, A.grad[q][i], m, v, A.a[q]);
-    A.em[q][i] = m; A.ev[q][i] = v;
-  }
-}
-
-// d c2w of every keyframe block (one CTA per frame)
-__global__ void pose_grad_frames_kernel(const float* __restrict__ dirs, const float* __restrict__ dro, const float* __restrict__ drd,
-                                        const int32_t* __restrict__ offs, float* __restrict__ out) {
-  __shared__ double red[32];
-  const int lo = offs[blockIdx.x], hi = offs[blockIdx.x + 1];
-  double acc[12];
-#pragma unroll
-  for (int k = 0; k < 12; k++) acc[k] = 0.0;
-  for (int r = lo + threadIdx.x; r < hi; r += blockDim.x) {
-#pragma unroll
-    for (int i = 0; i < 3; i++) {
-      const double g = (double)drd[3 * r + i];
-#pragma unroll
-      for (int j = 0; j < 3; j++) acc[4 * i + j] += g * (double)dirs[3 * r + j];
-      acc[4 * i + 3] += (double)dro[3 * r + i];
-    }
-  }
-  for (int k = 0; k < 12; k++) { const double t = block_sum(acc[k], red); if (threadIdx.x == 0) out[12 * blockIdx.x + k] = (float)t; }
+  adam_voxel_group(A.g[q], A.slots[q], A.grad[q], A.em[q], A.ev[q], A.a[q], b - A.blk0[q], A.blk0[q + 1] - A.blk0[q]);
 }
 
 }  // namespace nsb
@@ -608,14 +553,14 @@ extern "C" int nsb_copy_block(void* dst, const void* src, size_t bytes, void* st
 
 extern "C" int nsb_pose_grad(const float* dirs, const float* d_rays_o, const float* d_rays_d, int n, double* d_c2w, void* stream) {
   if (n < 0 || !d_c2w || (n > 0 && (!dirs || !d_rays_o || !d_rays_d))) { set_error("pose_grad: bad arguments"); return NSB_ERR_ARG; }
-  pose_grad_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, n, d_c2w, nullptr, no_peers());
+  pose_grad_kernel<double><<<1, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, nullptr, n, d_c2w, nullptr, no_peers());
   return check_cuda(cudaGetLastError(), "pose_grad launch");
 }
 extern "C" int nsb_pose_grad_peers(const float* dirs, const float* d_rays_o, const float* d_rays_d, int n, const double* loss_local,
                                    double* loss_and_d_c2w, const nsb_peers* peers, void* stream) {
   if (n < 0 || !loss_and_d_c2w || (n > 0 && (!dirs || !d_rays_o || !d_rays_d))) { set_error("pose_grad_peers: bad arguments"); return NSB_ERR_ARG; }
   PeerX px; int rc = make_peers(peers, &px); if (rc) return rc;
-  pose_grad_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, n, loss_and_d_c2w, loss_local, px);
+  pose_grad_kernel<double><<<1, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, nullptr, n, loss_and_d_c2w, loss_local, px);
   return check_cuda(cudaGetLastError(), "pose_grad_peers launch");
 }
 
@@ -662,13 +607,9 @@ static int adam_scalars(double lr, double beta1, double beta2, double eps, int s
 }
 extern "C" int nsb_adam_masked_voxels(const nsb_grid* grid, const int32_t* slot_map, const float* grad, float* exp_avg, float* exp_avg_sq,
                                       double lr, double beta1, double beta2, double eps, int step, void* stream) {
-  if (!grid || !grid->data || !slot_map || !grad || !exp_avg || !exp_avg_sq || grid->D < 1 || grid->H < 1 || grid->W < 1) {
-    set_error("adam_masked_voxels: bad arguments"); return NSB_ERR_ARG; }
-  AdamScalars a; int rc = adam_scalars(lr, beta1, beta2, eps, step, &a); if (rc) return rc;
-  const long long n = (long long)grid->D * grid->H * grid->W;
-  const int blocks = (int)((n + 7) / 8 < 148 * 16 ? (n + 7) / 8 : 148 * 16);
-  adam_masked_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(*grid, slot_map, grad, exp_avg, exp_avg_sq, a);
-  return check_cuda(cudaGetLastError(), "adam_masked_voxels launch");
+  if (!grid) { set_error("adam_masked_voxels: bad arguments"); return NSB_ERR_ARG; }
+  const nsb_adam_voxel_group G = {*grid, slot_map, grad, exp_avg, exp_avg_sq, lr, step};
+  return nsb_adam_mapper_step_decoders(&G, 1, nullptr, 0, beta1, beta2, eps, stream);
 }
 static int adam_table(int level, const nsb_decoder_params* p, AdamTable* Tp) {
   AdamTable& T = *Tp; memset(&T, 0, sizeof(T));
@@ -687,11 +628,8 @@ static int adam_table(int level, const nsb_decoder_params* p, AdamTable* Tp) {
 }
 extern "C" int nsb_adam_decoder(int level, const nsb_decoder_params* p, const float* grad_flat, float* exp_avg, float* exp_avg_sq,
                                 double lr, double beta1, double beta2, double eps, int step, void* stream) {
-  if (level < 0 || level > 3 || !p || !grad_flat || !exp_avg || !exp_avg_sq) { set_error("adam_decoder: bad arguments"); return NSB_ERR_ARG; }
-  AdamScalars a; int rc = adam_scalars(lr, beta1, beta2, eps, step, &a); if (rc) return rc;
-  AdamTable T; if ((rc = adam_table(level, p, &T))) return rc;
-  adam_flat_kernel<<<32, 256, 0, (cudaStream_t)stream>>>(T, grad_flat, exp_avg, exp_avg_sq, a);
-  return check_cuda(cudaGetLastError(), "adam_decoder launch");
+  const nsb_adam_decoder_item d = {level, p, grad_flat, exp_avg, exp_avg_sq, lr, step};
+  return nsb_adam_mapper_step_decoders(nullptr, 0, &d, 1, beta1, beta2, eps, stream);
 }
 extern "C" int nsb_adam_mapper_step(const nsb_adam_voxel_group* groups, int n_groups, int dec_level, const nsb_decoder_params* dec_params,
                                     const float* dec_grad_flat, float* dec_exp_avg, float* dec_exp_avg_sq, double dec_lr, int dec_step,
@@ -861,7 +799,7 @@ extern "C" int nsb_pose_grad_frames(const float* dirs, const float* d_rays_o, co
                                     int n_frames, float* out, void* stream) {
   if (n_frames < 0 || (n_frames > 0 && (!dirs || !d_rays_o || !d_rays_d || !frame_offsets || !out))) { set_error("pose_grad_frames: bad arguments"); return NSB_ERR_ARG; }
   if (n_frames == 0) return NSB_OK;
-  pose_grad_frames_kernel<<<n_frames, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, frame_offsets, out);
+  pose_grad_kernel<float><<<n_frames, 256, 0, (cudaStream_t)stream>>>(dirs, d_rays_o, d_rays_d, frame_offsets, 0, out, nullptr, no_peers());
   return check_cuda(cudaGetLastError(), "pose_grad_frames launch");
 }
 

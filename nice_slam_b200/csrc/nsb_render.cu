@@ -776,17 +776,7 @@ __device__ __forceinline__ bool fused_pose_grad(const KParams& P, int n_writers,
   if (!s_pose_last) return false;
   __threadfence();
   double acc[12];
-#pragma unroll
-  for (int k = 0; k < 12; k++) acc[k] = 0.0;
-  for (int r = threadIdx.x; r < P.in.n_rays; r += blockDim.x) {
-#pragma unroll
-    for (int i = 0; i < 3; i++) {
-      const double g = (double)__ldcg(P.bw.d_rays_d + 3 * r + i);
-#pragma unroll
-      for (int j = 0; j < 3; j++) acc[4 * i + j] += g * (double)__ldg(P.bw.pose_dirs + 3 * r + j);
-      acc[4 * i + 3] += (double)__ldcg(P.bw.d_rays_o + 3 * r + i);
-    }
-  }
+  pose_grad_partial(P.bw.pose_dirs, P.bw.d_rays_o, P.bw.d_rays_d, 0, P.in.n_rays, acc);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 #pragma unroll
   for (int k = 0; k < 12; k++) {

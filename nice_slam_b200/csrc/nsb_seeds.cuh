@@ -1,5 +1,5 @@
-// nsb_seeds.cuh -- device bodies of the loss-seed computations (Tracker.py:108-123, Mapper.py:487-493) and the peer-memory exchange
-// helpers.  Used by the stand-alone single-CTA kernels of nsb_aux.cu and, fused, by the LAST CTA of the forward render kernels
+// nsb_seeds.cuh -- device bodies of the loss-seed computations (Tracker.py:108-123, Mapper.py:487-493), the d c2w sums and the peer-memory
+// exchange helpers.  Used by the stand-alone single-CTA kernels of nsb_aux.cu and, fused, by the LAST CTA of the render kernels
 // (nsb_render.cu): for small batches the loss seeds are produced by the forward launch itself.
 #pragma once
 // NOTE: no __restrict__ in this header.  These bodies communicate between threads through `scratch` / `res` across __syncthreads() and, in the
@@ -129,6 +129,21 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
   }
   __syncthreads();
   return t;   // valid in thread 0
+}
+// This thread's share of d c2w = [sum_r d_rays_d[r] (x) dirs[r] | sum_r d_rays_o[r]] over rows lo + threadIdx.x, step blockDim.x, below hi:
+// acc[4 i + j] (j < 3) and acc[4 i + 3].  The ray gradients are read through L2 (__ldcg): in the fused form other CTAs of the launch wrote them.
+__device__ __forceinline__ void pose_grad_partial(const float* dirs, const float* d_rays_o, const float* d_rays_d, int lo, int hi, double acc[12]) {
+#pragma unroll
+  for (int k = 0; k < 12; k++) acc[k] = 0.0;
+  for (int r = lo + threadIdx.x; r < hi; r += blockDim.x) {
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+      const double g = (double)__ldcg(d_rays_d + 3 * r + i);
+#pragma unroll
+      for (int j = 0; j < 3; j++) acc[4 * i + j] += g * (double)__ldg(dirs + 3 * r + j);
+      acc[4 * i + 3] += (double)__ldcg(d_rays_o + 3 * r + i);
+    }
+  }
 }
 __device__ __forceinline__ double sgn(double x) { return (x > 0.0) - (x < 0.0); }
 

@@ -195,33 +195,13 @@ class ShardedTrackingIteration:
 
     def build_graph(self, host_io=False):
         """CUDA graph of enqueue() (and, with host_io, of the pinned-host copies around it); None if capture fails."""
+        from .steps import capture_graph, host_io_body
         x = self.ctx
-
-        sm = host_io in ("sm", "sm_push")
-
-        def body():
-            if sm:                                                 # the blocks moved by nsb_copy_block launches over the mapped host views
-                x.copy_in_sm()
-            elif host_io:
-                x.d_in.copy_(x.h_in, non_blocking=True)
-            push = host_io == "sm_push" and self.peers is not None and self.fused       # the summing CTA stores [loss | d c2w] to pinned memory itself
-            self.enqueue(out13_ptr=x._mapped(x.h_pose13) if push else None)
-            if sm and not push:
-                x.copy_out_sm(x.h_pose13, self.packed)
-            elif host_io and not sm:
-                x.h_pose13.copy_(self.packed, non_blocking=True)
+        # sm_push: the summing CTA of the fused form stores [loss | d c2w] to pinned memory itself
+        body = host_io_body(x, host_io, self.packed, x.h_pose13, self.peers is not None and self.fused,
+                            lambda push: self.enqueue(out13_ptr=x._mapped(x.h_pose13) if push else None))
         try:
-            cur = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                body(); body()
-            cur.wait_stream(side)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
-            return g
+            return capture_graph(body)
         except Exception:
             torch.cuda.synchronize()
             return None
@@ -282,18 +262,10 @@ class ShardedMappingIteration:
         return reduce_sum(x.packed)
 
     def build_graph(self):
+        """CUDA graph of enqueue(); None if capture fails."""
+        from .steps import capture_graph
         try:
-            cur = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                self.enqueue(); self.enqueue()
-            cur.wait_stream(side)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.enqueue()
-            return g
+            return capture_graph(self.enqueue)
         except Exception:
             torch.cuda.synchronize()
             return None

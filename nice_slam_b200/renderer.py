@@ -359,7 +359,7 @@ class FusedRenderer(object):
     # ------------------------------------------------------------------ helpers
     def invalidate_decoders(self, levels=None):
         """Force a re-pack of the decoders' packed / operand images on the next call (needed only after parameter updates that bypass
-        torch's version counters, e.g. optim.FusedMapperAdam.step_decoder)."""
+        torch's version counters, e.g. optim.FusedMapperAdam.step_all)."""
         for lvl in (levels or list(self._cache.key.keys())):
             self._cache.key.pop(lvl, None)
 

@@ -36,6 +36,39 @@ def packed_layout(n_frames, grad_decoders, masked_counts):
     return sect, off
 
 
+def capture_graph(body):
+    """CUDA graph of one call of `body`, after two warm-up calls outside capture (lazy attribute setup, decoder packing)."""
+    cur = torch.cuda.current_stream()
+    side = torch.cuda.Stream()
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        body(); body()
+    cur.wait_stream(side)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        body()
+    return g
+
+
+def host_io_body(ctx, host_io, d_result, h_result, can_push, enqueue):
+    """Graph body: enqueue(push) between the move of ctx's input block from pinned host memory and the move of d_result to the pinned block
+    h_result (host_io: see IterationContext.build_graph).  push = "sm_push" and can_push: the launch that completes d_result stores it itself."""
+    sm, push = host_io in ("sm", "sm_push"), host_io == "sm_push" and can_push
+
+    def body():
+        if sm:
+            ctx.copy_in_sm()
+        elif host_io:
+            ctx.d_in.copy_(ctx.h_in, non_blocking=True)
+        enqueue(push)
+        if sm and not push:
+            ctx.copy_out_sm(h_result, d_result)
+        elif host_io and not sm:
+            h_result.copy_(d_result, non_blocking=True)
+    return body
+
+
 class IterationContext:
     def __init__(self, renderer, n_rays, stage, device, kind="track", grad_grids=(), grad_decoders=(), coarse_mapper=False,
                  masked=None, n_frames=0, host_staging=True):
@@ -261,31 +294,9 @@ class IterationContext:
         input block as for "sm", the result block stored to pinned memory by the backward's last CTA (needs dirs; else as "sm").
         Re-capture after anything that changes pointers (grids re-created) or the decoders' packed image."""
         ro, rd, gd, gc = self.device_views()
-
-        sm = host_io in ("sm", "sm_push")
-
-        def body():
-            if sm:
-                self.copy_in_sm()                                          # the input block moved by one nsb_copy_block launch over the mapped host view
-            elif host_io:
-                self.d_in.copy_(self.h_in, non_blocking=True)             # one H2D copy: rays, sensor depth and colour
-            push = host_io == "sm_push" and dirs is not None          # the backward's last CTA stores the result block to pinned memory itself
-            self.run(c, decoders, ro, rd, gd, gc, dirs=dirs, result_to_host=push, **kw)     # d c2w comes out of the backward kernel
-            if sm and not push:
-                self.copy_out_sm()
-            elif host_io and not sm:
-                self.h_res.copy_(self.d_res, non_blocking=True)           # one D2H copy: ray gradients, loss, pose gradient
-        cur = torch.cuda.current_stream()
-        side = torch.cuda.Stream()
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            body(); body()                       # warm-up outside capture: lazy attribute setup, decoder packing
-        cur.wait_stream(side)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            body()
-        return g
+        body = host_io_body(self, host_io, self.d_res, self.h_res, dirs is not None,
+                            lambda push: self.run(c, decoders, ro, rd, gd, gc, dirs=dirs, result_to_host=push, **kw))
+        return capture_graph(body)
 
     def _mapped(self, t):
         """Device view of a pinned host tensor (nsb_host_device_pointer); resolved once, outside any graph capture."""
@@ -304,9 +315,8 @@ class IterationContext:
         """h_in (pinned) -> d_in by nsb_copy_block on the current stream."""
         _lib.check(_lib.lib().nsb_copy_block(_VP(self.d_in.data_ptr()), _VP(self._mapped(self.h_in)), self.d_in.numel(), _stream()), "nsb_copy_block")
 
-    def copy_out_sm(self, dst=None, src=None):
-        """d_res -> h_res (pinned) by nsb_copy_block on the current stream (dst / src: another pinned / device pair of equal size)."""
-        dst, src = (self.h_res, self.d_res) if dst is None else (dst, src)
+    def copy_out_sm(self, dst, src):
+        """src (device) -> dst (pinned, of equal size) by nsb_copy_block on the current stream."""
         _lib.check(_lib.lib().nsb_copy_block(_VP(self._mapped(dst)), _VP(src.data_ptr()), src.numel() * src.element_size(), _stream()), "nsb_copy_block")
 
     def stage_host_inputs(self, rays_o, rays_d, gt_depth, gt_color):

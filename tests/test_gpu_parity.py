@@ -762,8 +762,8 @@ def test_frustum_mask_matches_real_mapper_masks():
         assert MaskedVoxels(c[key], got.to(DEV)).count == int(got.sum())
 
 
-def test_fused_adam_matches_torch_adam():
-    """nsb_adam_masked_voxels / nsb_adam_decoder against torch.optim.Adam on the reference's parameterisation (val_grad = val[mask] as a
+def test_fused_adam_step_all_matches_torch_adam():
+    """FusedMapperAdam.step_all (one voxel group + the colour decoder) against torch.optim.Adam on the reference's parameterisation (val_grad = val[mask] as a
     leaf, the colour decoder's parameters), three steps with changing gradients and learning rates (Mapper.py:365-379, :412-419, :504)."""
     from nice_slam_b200._lib import LEVELS, flat_layout
     from nice_slam_b200.masked import MaskedVoxels
@@ -792,8 +792,7 @@ def test_fused_adam_matches_torch_adam():
         for name, off, cnt in lay:
             dec_ref[name].grad = gflat[off:off + cnt].view_as(dec_ref[name]).clone()
         opt.step()
-        fused.step_voxels(key, c[key], mv, gv, lr_v)
-        fused.step_decoder("color", dec, gflat, lr_d, renderer=renderer)
+        fused.step_all([(key, c[key], mv, gv, lr_v)], [("color", dec, gflat, lr_d)], renderer=renderer)
         want = val_ref.clone()
         want[mask5] = val_grad.detach()
         assert rel(c[key], want) < 1e-6, step
