@@ -80,8 +80,12 @@ int nsb_version(void);
 const char* nsb_last_error(void);
 /* Process-wide options.  "mlp_backend": 0 = auto (default: tensor-core tile kernels), 1 = FP32-FMA decoders, 2 = tensor-core round-1 ray-group
  * kernels, 3 = tensor-core tile kernels (wgmma 3xTF32, two CTAs per SM).  "split_model": 1 (default) = a tile's decoders are spread over CTAs only while
- * that beats one CTA per tile by wave efficiency, 0 = always for batches of <= 262144 points.  "wgrad_tc", "fwd_f16", "pdl", "small_rays": DESIGN.md. */
+ * that beats one CTA per tile by wave efficiency, 0 = always for batches of <= 262144 points.  "wgrad_all": 0 (default) = only fine / colour
+ * decoder weight gradients take the tensor cores, 1 = any decoders' (middle and coarse too) whose layer outputs the forward kept
+ * (nsb_forward_outputs.acts_levels may then name them).  "wgrad_tc", "fwd_f16", "pdl", "small_rays": DESIGN.md. */
 int nsb_set_option(const char* key, int value);
+/* Current value of an option of nsb_set_option -> *value (NSB_ERR_ARG for an unknown key). */
+int nsb_get_option(const char* key, int* value);
 
 /* Diagnostic: resident CTAs per SM of the tile-centric tensor-core kernels (2 = the design point: two tiles in flight per SM). */
 int nsb_debug_occupancy(int* fwd_ctas_per_sm, int* bwd_ctas_per_sm);
@@ -141,9 +145,10 @@ typedef struct {
                                     gradients the backward will be asked for (acts_levels).  When the forward keeps them, the backward computes
                                     those weight gradients on the tensor cores (dW = dU^T X contracted over the points of a tile) instead of the
                                     FP32-FMA pass that recomputes the forward.  NULL = not kept. */
-  int acts_levels;               /* which decoders' layer outputs `acts` holds: bit (1 << NSB_FINE) and / or (1 << NSB_COLOR), decoders of the
-                                    stage only, one [N,S,5,32] block each in level order (fine first).  0 = the colour decoder in stage color,
-                                    nothing otherwise (src/Mapper.py:339-341 with fix_fine; fix_fine = False adds the fine decoder). */
+  int acts_levels;               /* which decoders' layer outputs `acts` holds: bit (1 << NSB_FINE) and / or (1 << NSB_COLOR) -- with option
+                                    "wgrad_all" also (1 << NSB_MIDDLE) / (1 << NSB_COARSE) --, decoders of the stage only, one [N,S,5,32] block
+                                    each in level order (coarse, middle, fine, colour).  0 = the colour decoder in stage color, nothing
+                                    otherwise (src/Mapper.py:339-341 with fix_fine; fix_fine = False adds the fine decoder). */
 } nsb_forward_outputs;
 
 /* Bytes of nsb_forward_outputs.split_workspace for n_rays rays of n_samples_total samples; non-zero for every n_rays >= 1 (0 for

@@ -80,6 +80,7 @@ SYMBOLS = {
     "nsb_version": (C.c_int, []),
     "nsb_last_error": (C.c_char_p, []),
     "nsb_set_option": (C.c_int, [C.c_char_p, C.c_int]),
+    "nsb_get_option": (C.c_int, [C.c_char_p, C.POINTER(C.c_int)]),
     "nsb_debug_occupancy": (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "nsb_flat_decoder_floats": (C.c_size_t, [C.c_int]),
     "nsb_flat_offset": (C.c_longlong, [C.c_int, C.c_int, C.c_int]),
@@ -157,6 +158,9 @@ def lib():
         wg = os.environ.get("NSB_WGRAD_TC")                  # 0 = decoder weight gradients by the FP32-FMA pass (default: tensor cores)
         if wg is not None:
             h.nsb_set_option(b"wgrad_tc", int(wg))
+        wa = os.environ.get("NSB_WGRAD_ALL")                 # 1 = middle / coarse decoder weight gradients on the tensor cores too (default: 0)
+        if wa is not None:
+            h.nsb_set_option(b"wgrad_all", int(wa))
         pdl = os.environ.get("NSB_PDL")                      # 0 = plain stream order between the forward and backward launches of an iteration
         if pdl is not None:
             h.nsb_set_option(b"pdl", int(pdl))
@@ -174,6 +178,13 @@ def check(rc, what):
     if rc != 0:
         msg = lib().nsb_last_error().decode("utf-8", "replace")
         raise RuntimeError("nice_slam_b200.%s failed (status %d): %s" % (what, rc, msg))
+
+
+def get_option(name):
+    """Current value of a library option (nsb_get_option)."""
+    v = C.c_int(0)
+    check(lib().nsb_get_option(name.encode(), C.byref(v)), "nsb_get_option(%s)" % name)
+    return v.value
 
 
 def flat_layout(level):

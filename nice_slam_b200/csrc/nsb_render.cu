@@ -1073,12 +1073,20 @@ static int weight_bytes(const int* dec, int n) {
   return wb;
 }
 
-// nsb_forward_outputs / nsb_backward_args .acts_levels -> K.acts_mask (0 keeps fill_common's default): the fine and colour decoders of the stage
+static int g_wgrad_all = 0;        // weight gradients of every decoder (middle and coarse too) on the tensor cores when the forward kept their layer outputs
+
+// nsb_forward_outputs / nsb_backward_args .acts_levels -> K.acts_mask (0 keeps fill_common's default): the fine and colour decoders of the stage,
+// with option wgrad_all any decoder of the stage
 static int apply_acts_levels(KParams& K, int levels) {
   if (levels == 0) return NSB_OK;
   int stage_mask = 0; for (int i = 0; i < K.n_dec; i++) stage_mask |= 1 << K.dec[i];
-  if ((levels & ~((1 << NSB_FINE) | (1 << NSB_COLOR))) || (levels & ~stage_mask)) {
-    set_error("acts_levels 0x%x: only the fine / colour decoders of the stage keep layer outputs", levels); return NSB_ERR_ARG; }
+  const int allowed = g_wgrad_all ? 0xf : (1 << NSB_FINE) | (1 << NSB_COLOR);
+  if ((levels & ~allowed) || (levels & ~stage_mask)) {
+    set_error(g_wgrad_all ? "acts_levels 0x%x: only decoders of the stage keep layer outputs"
+                          : "acts_levels 0x%x: only the fine / colour decoders of the stage keep layer outputs (middle / coarse: option wgrad_all)",
+              levels);
+    return NSB_ERR_ARG;
+  }
   K.acts_mask = levels;
   return NSB_OK;
 }
@@ -1261,6 +1269,7 @@ static int set_attrs() {
     {(const void*)render_fwd_tile_sampled_kernel, tile_smem_bytes(false), true, "render_fwd_tile_sampled_kernel"},
     {(const void*)render_bwd_tile_kernel, tile_smem_bytes(true), true, "render_bwd_tile_kernel"},
     {(const void*)render_bwd_wg_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_tile_kernel"},
+    {(const void*)render_bwd_wg_coarse_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_coarse_tile_kernel"},
   };
   for (const auto& a : attrs)
     if (check_cuda(cudaFuncSetAttribute(a.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)a.smem), a.name) ||
@@ -1314,11 +1323,21 @@ using namespace nsb;
 
 extern "C" int nsb_set_option(const char* key, int value) {
   if (key && !strcmp(key, "wgrad_tc")) { g_wgrad_tc = value != 0; return NSB_OK; }
+  if (key && !strcmp(key, "wgrad_all")) { g_wgrad_all = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "fwd_f16")) { g_fwd_f16 = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "pdl")) { g_pdl = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "split_model")) { g_split_model = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "small_rays")) { if (value < 0) { set_error("small_rays must be >= 0"); return NSB_ERR_ARG; } g_small_rays = value; return NSB_OK; }
   if (key && !strcmp(key, "mlp_backend")) { if (value < 0 || value > 3) { set_error("mlp_backend must be 0 (auto = tile kernels), 1 (FP32-FMA), 2 (round-1 ray-group tensor-core kernels) or 3 (tensor-core tile kernels)"); return NSB_ERR_ARG; } g_mlp_backend = value; return NSB_OK; }
+  set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
+}
+
+extern "C" int nsb_get_option(const char* key, int* value) {
+  if (!value) { set_error("nsb_get_option: value is NULL"); return NSB_ERR_ARG; }
+  const struct { const char* name; int v; } opts[] = {{"wgrad_tc", g_wgrad_tc}, {"wgrad_all", g_wgrad_all}, {"fwd_f16", g_fwd_f16}, {"pdl", g_pdl},
+                                                      {"split_model", g_split_model}, {"small_rays", g_small_rays}, {"mlp_backend", g_mlp_backend}};
+  for (const auto& o : opts)
+    if (key && !strcmp(key, o.name)) { *value = o.v; return NSB_OK; }
   set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
 }
 
@@ -1451,7 +1470,8 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   if ((rc = fma_config(K, true, &warps, &smem))) return rc;
   // Plan: with the saved ReLU masks a tensor-core launch for the decoders that only need input gradients (rays, voxels), then one for those
   // whose WEIGHT gradients are requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341; with fix_fine = False also the
-  // fine decoder): on the tensor cores when they are fine / colour decoders whose layer outputs the forward kept (acts; one CTA per SM), else
+  // fine decoder; every decoder of the stage when the caller leaves them all trainable, as the tracker and mapper do): on the tensor cores when
+  // they are fine / colour decoders -- with option wgrad_all any decoders -- whose layer outputs the forward kept (acts; one CTA per SM), else
   // FP32-FMA, which recomputes the forward.  Without masks, or on the FP32-FMA back-end, one FP32-FMA launch for every decoder.
   enum Kind { TileIg, GroupIg, WgTile, Fma };
   const Family fam = kernel_family(K.S, in->n_rays, false);
@@ -1467,7 +1487,8 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     }
     if (ig.n_dec > 0) { L[n] = ig; kind[n++] = fam == Family::Tile ? TileIg : GroupIg; }
     bool wg_tc = wg.n_dec > 0 && bw->acts != nullptr && fam == Family::Tile && g_wgrad_tc && !sharded;
-    for (int i = 0; i < wg.n_dec; i++) wg_tc = wg_tc && (wg.dec[i] == NSB_FINE || wg.dec[i] == NSB_COLOR) && ((K.acts_mask >> wg.dec[i]) & 1);
+    for (int i = 0; i < wg.n_dec; i++)
+      wg_tc = wg_tc && (g_wgrad_all || wg.dec[i] == NSB_FINE || wg.dec[i] == NSB_COLOR) && ((K.acts_mask >> wg.dec[i]) & 1);
     if (wg.n_dec > 0) { L[n] = wg; kind[n++] = wg_tc ? WgTile : Fma; }       // (every decoder here: wg == K)
   }
   // Every launch after the first adds to the ray gradients; the last one writes d c2w from its last CTA (the FP32-FMA kernel does not:
@@ -1484,7 +1505,10 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     if (kind[i] == GroupIg) rc = launch_group(P, true, bw->split_workspace, bw->split_workspace_bytes, st);
     else if (kind[i] == Fma) rc = launch_fma(P, true, st);
     else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true))) return rc;
-    else if (kind[i] == WgTile) {
+    else if (kind[i] == WgTile && P.dec[0] == NSB_COARSE) {         // (stage coarse: the coarse decoder alone)
+      render_bwd_wg_coarse_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
+      rc = check_cuda(cudaGetLastError(), "render_bwd_wg_coarse_tile_kernel launch");
+    } else if (kind[i] == WgTile) {
       render_bwd_wg_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
       rc = check_cuda(cudaGetLastError(), "render_bwd_wg_tile_kernel launch");
     } else if (after_forward && !any_w && g_pdl) {

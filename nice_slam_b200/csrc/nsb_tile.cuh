@@ -616,8 +616,8 @@ __device__ __forceinline__ void epi_forward(const KParams& P, const TileSmem& t,
   NSB_PH(12);
 }
 
-// ---- tensor-core weight gradients (the colour decoder in the mapper's colour stage, src/Mapper.py:339-341,503, and the fine decoder with -----
-// fix_fine = False) ---------------------------------------------------------------------------------------------------------------------
+// ---- tensor-core weight gradients (the colour decoder in the mapper's colour stage, src/Mapper.py:339-341,503, the fine decoder with ---------
+// fix_fine = False; with option wgrad_all also the middle and coarse decoders, which the tracker's and mapper's autograd ask for) -----------
 // dW_i = DU_i^T X_i, dWc_i = G_i^T C, dWo = g_out^T H_4, dB = P^T DX are contractions over the POINTS of a tile: both operands of the MMA have the
 // points as K.  wgmma takes tf32 operands K-major only, so the epilogue threads write the rows they own a second time, transposed, into
 // [feature][point] tiles (the canonical no-swizzle layout with K = 128 points): DU_i and G_i form the A operand (M = 64 = [DU | G], hi tiles
@@ -630,14 +630,18 @@ constexpr int kWgALo = 2 * kMnTile, kWgBLo = kMnTile;          // offsets of the
 struct WgSmem { float* du; float* g; float* b; float* dpk; };
 // block of decoder lv in fo.acts / bw.acts (levels of `mask` in level order), -1 if its layer outputs are not kept
 __host__ __device__ __forceinline__ int acts_slot(int mask, int lv) { return (mask >> lv) & 1 ? __builtin_popcount(mask & ((1 << lv) - 1)) : -1; }
-// packed-gradient offsets of the two weight-gradient decoders: fine (fc_c input [c_fine | c_middle], 64 wide; one output) and colour (32; four)
+// packed-gradient offsets of a weight-gradient decoder: fine (fc_c input [c_fine | c_middle], 64 wide; one output), colour (32; four), middle
+// (32; one) and coarse (no embedding, no fc_c: layer 0 and the skip part of layer 3 read the coarse features, 32 wide; one output)
 struct WgDec { int o_W0, o_W1, o_W2, o_W3E, o_W3H, o_W4, o_WC, PC, o_WO, no, o_b, o_bc, o_bo; };
 template <int LV>
 __device__ __forceinline__ WgDec wg_dec() {
   using D = Dec<LV>;
   return WgDec{D::o_W0, D::o_W1, D::o_W2, D::o_W3E, D::o_W3H, D::o_W4, D::o_WC, D::PC, D::o_WO, D::NO, D::o_b, D::o_bc, D::o_bo};
 }
-static_assert(Dec<2>::PH == Dec<3>::PH && Dec<2>::PF == Dec<3>::PF && Dec<2>::o_B == Dec<3>::o_B, "shared pitches of the WG decoders");
+static_assert(Dec<0>::PH == Dec<3>::PH && Dec<1>::PH == Dec<3>::PH && Dec<2>::PH == Dec<3>::PH, "shared hidden pitch of the WG decoders");
+static_assert(Dec<1>::PF == Dec<3>::PF && Dec<2>::PF == Dec<3>::PF && Dec<1>::o_B == Dec<3>::o_B && Dec<2>::o_B == Dec<3>::o_B,
+              "shared first-input pitch and embedding block of the xyz WG decoders");
+static_assert(Dec<1>::o_WO == Dec<3>::o_WO && Dec<1>::o_bo == Dec<3>::o_bo && Dec<1>::TOTAL == Dec<3>::TOTAL, "middle decoder = colour layout");
 __device__ __forceinline__ void split4(const float4 v, float4& h, float4& l) {
   h = make_float4(tc::to_tf32(v.x), tc::to_tf32(v.y), tc::to_tf32(v.z), tc::to_tf32(v.w));
   l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
@@ -833,18 +837,25 @@ __device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, in
 // ---- backward of one decoder.  Leaves dL/dc rows ([128][32] fp32) in a[0] and the embedding-chain part of dL/dp ([128][4] fp32, row r at
 // a[1] + bwd_dpe_off(r)) in a[1]; the caller scatters after an epi_sync().  Each warpgroup writes both into its own rows of the operand tiles,
 // which only its own (completed) MMAs read.  masks = this decoder's ReLU-mask words of the tile's point 0 (point stride 15).
+// WG = which weight gradients the instantiation computes: none (input gradients only, any decoder), those of the xyz decoders (middle, fine,
+// colour) or those of the coarse decoder (no embedding, no fc_c).  The coarse decoder has its own instantiation: its branches compiled into
+// the xyz one took that kernel past 255 registers (spills).
+enum { kWgNone = 0, kWgXyz = 1, kWgCoarse = 2 };
 __device__ __forceinline__ int bwd_dpe_off(int r) { return (r >> 6) * (64 * 32) + (r & 63) * 4; }
-template <bool WG>
+template <int WG>
 __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t, Issuer& I, const BwdExtra& X, int lv, const PointGeom& G, int hb, uint32_t hdr_parity,
                                              const uint32_t* __restrict__ masks, int npts, int off0, long long gp0, WgSmem* w = nullptr, const float* acts_row = nullptr) {
   const int row = threadIdx.x & (TM - 1), cg = threadIdx.x >> 7, warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31, q = lane & 3;
   const int r0 = 64 * (threadIdx.x >> 7) + 16 * (warp & 3) + (lane >> 2);      // rows of this thread's fragment: r0 (elements e with bit 1 clear) and r0 + 8
   const int S = P.S;
-  constexpr int PH = Dec<3>::PH, PF = Dec<3>::PF;                 // (the same for both WG decoders)
-  const WgDec DW = lv == 2 ? wg_dec<2>() : wg_dec<3>();          // packed gradient image of this WG decoder
+  constexpr bool kWg = WG != kWgNone;
+  constexpr int PH = Dec<3>::PH, PF = WG == kWgCoarse ? Dec<0>::PF : Dec<3>::PF;      // (PH: the same for every WG decoder)
+  // packed gradient image of this WG decoder.  The middle decoder's is the colour decoder's layout with one output: rows 1..3 of dWo and
+  // dbo[1..3], padding of its image that the unpack does not read, receive the zero columns 1..3 of its g_out.
+  const WgDec DW = WG == kWgCoarse ? wg_dec<0>() : lv == 2 ? wg_dec<2>() : wg_dec<3>();
   float creg[kCW], cmid[kCW];                                    // WG: this thread's 16 grid features of its point (fine: + the middle grid's)
-  const bool xyz = lv != 0;
+  const bool xyz = WG == kWgCoarse ? false : lv != 0;
   const float* hdr = t.hdr + hb * kHdrFloats;
   // ReLU bits of this thread's elements: word i of a row shifted right by 2 q puts column 8 j + 2 q + k on bit 8 j + k; row r0 + 8 goes to bits
   // 8 j + 2 + k, and layers (0, 1) / (2, 3) share m01 / m23 (odd layer in the high nibble of each byte)
@@ -871,11 +882,11 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       d1[e] = v;
     }
   }
-  if constexpr (WG) {
+  if constexpr (kWg) {
     float g_out[4];
     bwd_gout(X, lv, row, npts, off0, S, g_out);
-    // grid features of this point -> registers (gathered once through the B tile)
-    gather_tile_kt(P.in.grid[lv], w->b, kWgBLo, G.xn, warp, lane);
+    // grid features of this point -> registers (gathered once through the B tile; the coarse grid at the enlarged coarse bound)
+    gather_tile_kt(P.in.grid[lv], w->b, kWgBLo, WG == kWgCoarse ? G.xnc : G.xn, warp, lane);
     __syncthreads();
     get_kt16(w->b, kWgBLo, row, cg, creg);
     __syncthreads();
@@ -917,23 +928,27 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       if (xyz) put2(t.a[0], r, c, d1[e], d1[e + 1]);
       put2(t.a[1], r, c, du[e], du[e + 1]);
     }
-    if constexpr (WG) {                                          // the same values transposed ([feature][point]) and their column sums: db_i, dbc_i
+    if constexpr (kWg) {                                         // the same values transposed ([feature][point]) and their column sums: db_i, dbc_i
 #pragma unroll
       for (int e = 0; e < 16; e++) {
         const int r = r0 + 8 * ((e >> 1) & 1), c = 8 * (e >> 2) + 2 * q + (e & 1);
-        put_kt1(w->du, kWgALo, c, r, du[e]); put_kt1(w->g, kWgALo, c, r, d1[e]);
+        put_kt1(w->du, kWgALo, c, r, du[e]);
+        if constexpr (WG != kWgCoarse) put_kt1(w->g, kWgALo, c, r, d1[e]);      // (the coarse decoder has no fc_c: no G block, no dbc)
       }
-      const float sb = frag_colsum(du, lane), sc = frag_colsum(d1, lane);
+      const float sb = frag_colsum(du, lane);
+      float sc = 0.0f;
+      if constexpr (WG != kWgCoarse) sc = frag_colsum(d1, lane);
       const int col = frag_colsum_col(lane);
-      atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb); atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
+      atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb);
+      if constexpr (WG != kWgCoarse) atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
     }
     fence_proxy_async();
     wg_bar_sync();                                               // this warpgroup's rows of G / DU are written -> its MMAs
     NSB_PH(22);
-    issue_bwd_layer(I, t, lv, i, d1, dc, fa);
+    issue_bwd_layer(I, t, WG == kWgCoarse ? 0 : lv, i, d1, dc, fa);
     if (threadIdx.x == 0) loader_top_up(I.L, t, I.issued);       // slots of this layer are free: fetch the next layer's units under the epilogue
     NSB_PH(23);
-    if constexpr (WG) {                                          // weight gradients of layer i
+    if constexpr (kWg) {                                         // weight gradients of layer i
       if (i >= 1) {                                              // hidden input H_{i-1}
         float xr[kCW];
 #pragma unroll
@@ -945,24 +960,31 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
         const int o_wh = i == 1 ? DW.o_W1 : i == 2 ? DW.o_W2 : i == 3 ? DW.o_W3H : DW.o_W4;
         wg_group(*w, 0, w->dpk + o_wh, PH, 32);
       }
-      put_kt16(w->b, kWgBLo, row, cg, creg);                             // dWc_i = G_i^T C
-      wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC, DW.PC, 32);
-      if (lv == 2) {                                             // fine: columns 32..63 of dWc_i = G_i^T C_middle (a second pass over the B tile)
-        put_kt16(w->b, kWgBLo, row, cg, cmid);
-        wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC + 32, DW.PC, 32);
+      if constexpr (WG != kWgCoarse) {
+        put_kt16(w->b, kWgBLo, row, cg, creg);                           // dWc_i = G_i^T C
+        wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC, DW.PC, 32);
+        if (lv == 2) {                                           // fine: columns 32..63 of dWc_i = G_i^T C_middle (a second pass over the B tile)
+          put_kt16(w->b, kWgBLo, row, cg, cmid);
+          wg_group(*w, 1, w->dpk + DW.o_WC + 32 * i * DW.PC + 32, DW.PC, 32);
+        }
       }
-      if (i == 3 || i == 0) {                                    // embedding part of W_0 / W_3
-        const float* B = hdr + 464;
-        for (int blk = 0; blk < 3; blk++) {
-          float e[kCW];
+      if (i == 3 || i == 0) {                                    // first-input part of W_0 / W_3: the embedding, or the coarse features
+        if constexpr (WG != kWgCoarse) {
+          const float* B = hdr + 464;
+          for (int blk = 0; blk < 3; blk++) {
+            float e[kCW];
 #pragma unroll
-          for (int j = 0; j < kCW; j++) {
-            const int f = 32 * blk + kCW * cg + j;
-            float x = G.pf[0] * B[f]; x = fmaf(G.pf[1], B[kEmbPad + f], x); x = fmaf(G.pf[2], B[2 * kEmbPad + f], x);
-            e[j] = f < kEmb ? __sinf(reduce_2pi(x)) : 0.0f;
+            for (int j = 0; j < kCW; j++) {
+              const int f = 32 * blk + kCW * cg + j;
+              float x = G.pf[0] * B[f]; x = fmaf(G.pf[1], B[kEmbPad + f], x); x = fmaf(G.pf[2], B[2 * kEmbPad + f], x);
+              e[j] = f < kEmb ? __sinf(reduce_2pi(x)) : 0.0f;
+            }
+            put_kt16(w->b, kWgBLo, row, cg, e);
+            wg_group(*w, 0, w->dpk + (i == 0 ? DW.o_W0 : DW.o_W3E) + 32 * blk, PF, 32);
           }
-          put_kt16(w->b, kWgBLo, row, cg, e);
-          wg_group(*w, 0, w->dpk + (i == 0 ? DW.o_W0 : DW.o_W3E) + 32 * blk, PF, 32);
+        } else {                                                 // coarse: dW_0 = DU_0^T C, dW_3[:, :32] = DU_3^T C
+          put_kt16(w->b, kWgBLo, row, cg, creg);
+          wg_group(*w, 0, w->dpk + (i == 0 ? DW.o_W0 : DW.o_W3E), PF, 32);
         }
       }
       NSB_PH(24);
@@ -978,7 +1000,7 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
   float dpe0[3] = {0.0f, 0.0f, 0.0f}, dpe1[3] = {0.0f, 0.0f, 0.0f};          // rows r0, r0 + 8
   if (xyz) {
     const float* B = hdr + 464;
-    if constexpr (WG) {                                          // B tile of the dB groups: the point's coordinates in columns 0..2
+    if constexpr (kWg) {                                         // B tile of the dB groups: the point's coordinates in columns 0..2
       float pv[kCW];
 #pragma unroll
       for (int j = 0; j < kCW; j++) pv[j] = (cg == 0 && j < 3) ? G.pf[j] : 0.0f;
@@ -1013,9 +1035,9 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
           dx = __cosf(reduce_2pi(x)) * fa[e];
           dpe[0] = fmaf(b0, dx, dpe[0]); dpe[1] = fmaf(b1, dx, dpe[1]); dpe[2] = fmaf(b2, dx, dpe[2]);
         }
-        if constexpr (WG) put_kt1(w->du, kWgALo, f - 32 * c, r0 + 8 * ((e >> 1) & 1), dx);
+        if constexpr (kWg) put_kt1(w->du, kWgALo, f - 32 * c, r0 + 8 * ((e >> 1) & 1), dx);
       }
-      if constexpr (WG) {                                        // dB[a][f] = sum_p p_a cos(.) dE_f  (embedder._B is a parameter of the decoder)
+      if constexpr (kWg) {                                       // dB[a][f] = sum_p p_a cos(.) dE_f  (embedder._B is a parameter of the decoder)
         const int nf = kEmb - 32 * c < 32 ? kEmb - 32 * c : 32;
         wg_group(*w, 0, w->dpk + Dec<3>::o_B + 32 * c, kEmbPad, nf, true);
       }
@@ -1230,9 +1252,10 @@ __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_sampled_kerne
 // ================================================================================================================================
 // backward kernel (input gradients: rays + grid voxels)
 // ================================================================================================================================
-// WG = true: the item's decoder (the colour or the fine decoder) also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the
-// "tensor-core weight gradients" helpers): 96 KB more shared memory in front of the common part -> one CTA per SM.
-template <bool WG>
+// WG != kWgNone: the item's decoder also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the "tensor-core weight
+// gradients" helpers; kWgXyz: the middle, fine and colour decoders, kWgCoarse: the coarse decoder): 96 KB more shared memory in front of the
+// common part -> one CTA per SM.
+template <int WG>
 __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using namespace tl;
@@ -1373,7 +1396,11 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   NSB_PH(32);
   if (fused_pose_grad(P, gridDim.x, reinterpret_cast<double*>(smem_raw))) pose_tail_peers(P);
 }
-__global__ void __launch_bounds__(tl::kThreads, 2) render_bwd_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<false>(P); }
-__global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<true>(P); }
+__global__ void __launch_bounds__(tl::kThreads, 2) render_bwd_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<tl::kWgNone>(P); }
+__global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<tl::kWgXyz>(P); }
+// the coarse decoder's weight gradients (stage coarse, option wgrad_all)
+__global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_coarse_tile_kernel(const __grid_constant__ KParams P) {
+  render_bwd_tile_body<tl::kWgCoarse>(P);
+}
 
 }  // namespace nsb

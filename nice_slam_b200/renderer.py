@@ -93,7 +93,7 @@ class _PackCache:
 class _Call:
     """Non-tensor arguments of one render call."""
     __slots__ = ("stage", "levels", "bound", "cbound", "n_samples", "n_surface", "gt_depth", "packed", "param_names",
-                 "aux", "masked", "grid_data", "lindisp", "t_rand", "z_given")
+                 "aux", "masked", "grid_data", "lindisp", "t_rand", "z_given", "grad_enabled")
 
 
 INLINE_MAX_RAYS = 1024          # NSB_INLINE_MAX_RAYS of include/nice_slam_b200.h
@@ -208,10 +208,12 @@ class _RenderFn(torch.autograd.Function):
         masks = torch.empty(n, S, 15, dtype=torch.int32, device=dev)      # ReLU sign bits: lets backward skip the forward recompute
         out.masks = masks.data_ptr()
         # decoders whose parameters need a gradient: when they are fine / colour decoders (the mapper's colour stage, Mapper.py:339-341, and the
-        # fine decoder with fix_fine = False) keep their layer outputs so that the backward computes the weight gradients on the tensor cores
+        # fine decoder with fix_fine = False), or any decoders with option wgrad_all, keep their layer outputs so that the backward computes the
+        # weight gradients on the tensor cores.  Only when a backward can follow: needs_input_grad is set under no_grad too (render_img with
+        # trainable decoders would otherwise keep 640 B per sample point and decoder that nobody reads).
         k0, graded = 3 + n_lvl, []
         for lvl in call.levels:
-            if any(ctx.needs_input_grad[k0 + i] for i in range(len(call.param_names[lvl]))):
+            if call.grad_enabled and any(ctx.needs_input_grad[k0 + i] for i in range(len(call.param_names[lvl]))):
                 graded.append(lvl)
             k0 += len(call.param_names[lvl])
         acts, acts_levels = acts_buffer(graded, call.levels, n, S, dev)
@@ -309,9 +311,10 @@ class _RenderFn(torch.autograd.Function):
 
 def acts_buffer(grad_decoders, levels, n, S, device):
     """(acts [k,n,S,5,32] float32 or None, acts_levels bit mask) for the stage decoders `levels` of which `grad_decoders` want weight gradients:
-    the tensor-core weight-gradient kernel serves a non-empty set of fine / colour decoders from their kept layer outputs."""
+    the tensor-core weight-gradient kernel serves a non-empty set of fine / colour decoders from their kept layer outputs, and with the
+    library option wgrad_all any non-empty set (the middle and coarse decoders too)."""
     wg = [lvl for lvl in LEVELS if lvl in grad_decoders and lvl in levels]
-    if not wg or not set(wg) <= {"fine", "color"}:
+    if not wg or not (set(wg) <= {"fine", "color"} or _lib.get_option("wgrad_all")):
         return None, 0
     return torch.empty(len(wg), n, S, 5, 32, dtype=torch.float32, device=device), sum(1 << LEVELS.index(lvl) for lvl in wg)
 
@@ -384,6 +387,7 @@ class FusedRenderer(object):
         call.aux = aux
         call.masked, call.grid_data = [None] * len(call.levels), [None] * len(call.levels)
         call.lindisp, call.t_rand, call.z_given = bool(self.lindisp), None, None
+        call.grad_enabled = torch.is_grad_enabled()           # (autograd.Function.forward itself always runs with grad mode off)
         grids = [c["grid_" + lvl] for lvl in call.levels]
         plist = [params[lvl][nm] for lvl in call.levels for nm in call.param_names[lvl]]
         return call, grids, plist

@@ -133,7 +133,7 @@ class IterationContext:
         self.d_flat = {lvl: self.packed[sect["dec_" + lvl][0]: sect["dec_" + lvl][0] + sect["dec_" + lvl][1]] for lvl in self.grad_decoders}
         # layer outputs of the fine / colour decoders, kept by the forward when their weight gradients are wanted: the backward then computes them
         # on the tensor cores (nsb_forward_outputs.acts / acts_levels); 640 B per sample point and decoder.  A set with the middle or coarse
-        # decoder takes the FP32-FMA pass, which reads no acts.
+        # decoder takes the FP32-FMA pass, which reads no acts, unless the library option wgrad_all is on (then every decoder's are kept).
         self.acts, self.acts_levels = acts_buffer(self.grad_decoders, self.levels, n, S, dev)
         self.buf = _lib.IterationBuffers(self.depth.data_ptr(), self.var.data_ptr(), self.rgb.data_ptr(), self.z_vals.data_ptr(),
                                          self.raw.data_ptr(), self.masks.data_ptr(), self.g_depth.data_ptr(), self.g_rgb.data_ptr(), self.loss.data_ptr(),
