@@ -329,6 +329,28 @@ int nsb_window_rays(const float* cams, const int32_t* cam_row, const float* fixe
 int nsb_adam_poses(float* cams, const int32_t* cam_row, int n_frames, const float* d_c2w, float* exp_avg, float* exp_avg_sq, float* d_cams,
                    double lr, double beta1, double beta2, double eps, int step, void* stream);
 
+/* ---- the tracker's per-frame camera loop (src/Tracker.py:71-128 optimize_cam_in_batch, :188-253 Tracker.run) ----------------------------------
+ * nsb_track_samples (one launch per iteration): n flat draws (int64, what torch.randint returns in select_uv, src/common.py:92-107) index the
+ * edge-cropped region rows [H0,H1) x columns [W0,W1) of a device-resident frame (depth float32 [H][W], colour float64 [H][W][3], the dtypes of
+ * the reference's frame loader): draw k is pixel i = W0 + k % (W1-W0), j = H0 + k / (W1-W0) (get_sample_uv, common.py:110-122).  Its ray comes
+ * from the camera tensor cam [7] as nsb_window_rays computes it (get_camera_from_tensor + get_rays_from_uv), depth / colour are read at [j, i],
+ * and the bbox pre-filter of nsb_bbox_prefilter (Tracker.py:95-104) decides whether it is kept.  Kept rays are written compacted in draw order
+ * (boolean indexing): rays_o, rays_d, dirs, gt_depth, gt_color [capacity n]; count[0] = rays kept; kept_index[p] (optional) = draw slot of
+ * kept ray p.  Draws must lie in [0, (H1-H0)(W1-W0)).
+ * nsb_track_pose_step (one launch per iteration): losses[step-1] = *loss; if *loss < best[0] (strict; the caller starts best = {1e10, -1},
+ * Tracker.py:223-247) then best = {loss, step-1} and candidate [7] := the camera tensor -- before this call's Adam step (post_step = 0: the
+ * reference's seperate_LR = True rebuilds the tensor by torch.cat each iteration) or after it (post_step = 1: seperate_LR = False steps the
+ * very tensor it later clones) -- and c2w16 := its pose as [4][4] float32 with the [0,0,0,1] row (Tracker.py:248-253).  d_c2w [3][4] (float64,
+ * the tracking iteration's) is rounded to float32, chained through quad2rotation and torch.optim.Adam steps cam in place: the quaternion at
+ * quat_lr, the translation at lr (Tracker.py:202-219), state exp_avg / exp_avg_sq [7]. */
+int nsb_track_samples(const float* cam, const int64_t* draws, int n, const float* depth, const double* color, int H, int W,
+                      int H0, int H1, int W0, int W1, double fx, double fy, double cx, double cy, const double bound[6],
+                      float* rays_o, float* rays_d, float* dirs, float* gt_depth, double* gt_color, int32_t* kept_index,
+                      int32_t* count, void* stream);
+int nsb_track_pose_step(float* cam, const double* loss, const double* d_c2w, float* exp_avg, float* exp_avg_sq, double lr, double quat_lr,
+                        double beta1, double beta2, double eps, int step, int post_step, double* losses, double* best,
+                        float* candidate, float* c2w16, void* stream);
+
 /* ---- exchanges of a ray-sharded tracking iteration through NVLink peer memory (SURVEY.md 8e) ---------------------------------
  * A batch sharded over `world` GPUs (equal shards) needs three batch-global quantities: max(gt_depth) (Renderer.py:109,144), the
  * median of the residuals (Tracker.py:113) and the sums of loss and pose gradient.  The *_peers variants of the three single-CTA

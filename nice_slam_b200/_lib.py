@@ -128,6 +128,10 @@ SYMBOLS = {
     "nsb_keyframe_gather": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "nsb_window_rays": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
     "nsb_adam_poses": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _P]),
+    "nsb_track_samples": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
+                                    C.c_double, C.c_double, C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
+    "nsb_track_pose_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int,
+                                      _P, _P, _P, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),
     "nsb_batch_max_depth_peers": (C.c_int, [_P, C.c_int, _P, C.POINTER(Peers), _P]),
     "nsb_tracking_seeds_peers": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(Peers), _P, _P, _P, _P, C.c_size_t, _P]),

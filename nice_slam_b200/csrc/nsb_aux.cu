@@ -237,13 +237,15 @@ __global__ void batch_max_kernel(const float* __restrict__ gt, int n, float* __r
 
 // ------------------------------------------------------------------------------------------------ ray pre-filter
 struct Bound6 { double b[6]; };
+__device__ __forceinline__ bool bbox_keep(const double* __restrict__ bound, const float o[3], const float d[3], float gt) {
+  return ray_far_bb(bound, o, d) >= (double)gt;    // Tracker.py:101 / Mapper.py:478
+}
 __global__ void prefilter_kernel(const float* __restrict__ ro, const float* __restrict__ rd, const float* __restrict__ gt,
                                  int n, const Bound6 B, uint8_t* __restrict__ keep) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float o[3] = {ro[3 * i], ro[3 * i + 1], ro[3 * i + 2]}, d[3] = {rd[3 * i], rd[3 * i + 1], rd[3 * i + 2]};
-  const double t = ray_far_bb(B.b, o, d);
-  keep[i] = (t >= (double)gt[i]) ? 1 : 0;          // Tracker.py:101 / Mapper.py:478
+  keep[i] = bbox_keep(B.b, o, d, gt[i]) ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------------ loss seeds
@@ -698,29 +700,31 @@ __global__ void window_poses_kernel(const float* __restrict__ cams, const int32_
   for (int k = 0; k < 12; k++) c2w_out[12 * f + k] = m[k];
 }
 // get_rays_from_uv (src/common.py:74-89): dirs = [(i-cx)/fx, -(j-cy)/fy, -1]; rays_d = sum_j dirs_j * R[:, j]; rays_o = t
+__device__ __forceinline__ void pixel_ray(const float* m, float pi, float pj, float fx, float fy, float cx, float cy,
+                                          float o[3], float d[3], float dir[3]) {
+  dir[0] = __fdiv_rn(__fsub_rn(pi, cx), fx); dir[1] = -__fdiv_rn(__fsub_rn(pj, cy), fy); dir[2] = -1.0f;
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    d[a] = __fadd_rn(__fadd_rn(__fmul_rn(dir[0], m[4 * a]), __fmul_rn(dir[1], m[4 * a + 1])), __fmul_rn(dir[2], m[4 * a + 2]));
+    o[a] = m[4 * a + 3];
+  }
+}
 __global__ void window_rays_kernel(const float* __restrict__ c2w, const float* __restrict__ pix_i, const float* __restrict__ pix_j,
                                    const int32_t* __restrict__ frame_of_ray, int n, float fx, float fy, float cx, float cy,
                                    float* __restrict__ rays_o, float* __restrict__ rays_d, float* __restrict__ dirs) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  const float* m = c2w + 12 * frame_of_ray[r];
-  const float d0 = __fdiv_rn(__fsub_rn(pix_i[r], cx), fx), d1 = -__fdiv_rn(__fsub_rn(pix_j[r], cy), fy), d2 = -1.0f;
+  float o[3], d[3], dir[3];
+  pixel_ray(c2w + 12 * frame_of_ray[r], pix_i[r], pix_j[r], fx, fy, cx, cy, o, d, dir);
 #pragma unroll
-  for (int a = 0; a < 3; a++) {
-    rays_d[3 * r + a] = __fadd_rn(__fadd_rn(__fmul_rn(d0, m[4 * a]), __fmul_rn(d1, m[4 * a + 1])), __fmul_rn(d2, m[4 * a + 2]));
-    rays_o[3 * r + a] = m[4 * a + 3];
-  }
-  if (dirs != nullptr) { dirs[3 * r] = d0; dirs[3 * r + 1] = d1; dirs[3 * r + 2] = d2; }
+  for (int a = 0; a < 3; a++) { rays_d[3 * r + a] = d[a]; rays_o[3 * r + a] = o[a]; }
+  if (dirs != nullptr) { dirs[3 * r] = dir[0]; dirs[3 * r + 1] = dir[1]; dirs[3 * r + 2] = dir[2]; }
 }
-// d camera tensor = (d c2w / d camera tensor)^T d c2w  (backward of get_camera_from_tensor), then torch.optim.Adam's update in place.
-// One thread per camera tensor (a window has <= a few dozen).  g: d c2w [3][4] of the tensor's window row.
-__global__ void adam_poses_kernel(float* __restrict__ cams, const int32_t* __restrict__ cam_row, int n_frames, const float* __restrict__ d_c2w,
-                                  float* __restrict__ em, float* __restrict__ ev, float* __restrict__ d_cams, const AdamScalars a) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n_frames || cam_row[f] < 0) return;
-  const int c = cam_row[f];
-  const float* g = d_c2w + 12 * f;
-  float* q = cams + 7 * c;
+// d camera tensor = (d c2w / d camera tensor)^T d c2w  (backward of get_camera_from_tensor), then torch.optim.Adam's update of the camera
+// tensor q in place: the quaternion q[0..3] with the scalars aq, the translation q[4..6] with at (the tracker's seperate_LR gives the
+// quaternion 0.2 x the learning rate, Tracker.py:211-213).  g: d c2w [3][4].  d_cams (optional): the camera-tensor gradient.
+__device__ __forceinline__ void pose_adam_step(float* __restrict__ q, const float* g, float* __restrict__ em, float* __restrict__ ev,
+                                               float* __restrict__ d_cams, const AdamScalars& aq, const AdamScalars& at) {
   const float r = q[0], i = q[1], j = q[2], k = q[3];
   const float nn = r * r + i * i + j * j + k * k, s = 2.0f / nn;
   const float G00 = g[0], G01 = g[1], G02 = g[2], G10 = g[4], G11 = g[5], G12 = g[6], G20 = g[8], G21 = g[9], G22 = g[10];
@@ -736,10 +740,104 @@ __global__ void adam_poses_kernel(float* __restrict__ cams, const int32_t* __res
 #pragma unroll
   for (int t = 0; t < 7; t++) {
     const float gr = dq[t];
-    if (d_cams != nullptr) d_cams[7 * c + t] = gr;
-    float m = em[7 * c + t], v = ev[7 * c + t];
-    q[t] = adam_update(q[t], gr, m, v, a);
-    em[7 * c + t] = m; ev[7 * c + t] = v;
+    if (d_cams != nullptr) d_cams[t] = gr;
+    float m = em[t], v = ev[t];
+    q[t] = adam_update(q[t], gr, m, v, t < 4 ? aq : at);
+    em[t] = m; ev[t] = v;
+  }
+}
+// One thread per camera tensor (a window has <= a few dozen); g: d c2w of the tensor's window row.
+__global__ void adam_poses_kernel(float* __restrict__ cams, const int32_t* __restrict__ cam_row, int n_frames, const float* __restrict__ d_c2w,
+                                  float* __restrict__ em, float* __restrict__ ev, float* __restrict__ d_cams, const AdamScalars a) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n_frames || cam_row[f] < 0) return;
+  const int c = cam_row[f];
+  pose_adam_step(cams + 7 * c, d_c2w + 12 * f, em + 7 * c, ev + 7 * c, d_cams != nullptr ? d_cams + 7 * c : nullptr, a, a);
+}
+
+// ---- the tracker's per-frame loop (Tracker.optimize_cam_in_batch, src/Tracker.py:71-128; Tracker.run's camera loop, :188-253) -----------------
+// Frame sampler, one CTA: flat draws k into the edge-cropped region (select_uv / get_sample_uv, common.py:92-134) -> pixel (i, j) -> rays of the
+// current camera tensor (get_camera_from_tensor + get_rays_from_uv) -> sensor depth / colour at [j, i] -> bbox pre-filter (Tracker.py:95-104),
+// kept rays compacted in draw order (what boolean indexing does).  count[0] = rays kept; kept_index (optional) = the draw slot of each kept ray.
+// (colour: float32 for the keyframe store, float64 as the tracker's frame loader delivers it)
+template <typename C>
+__device__ __forceinline__ void gather_pixel(const float* __restrict__ depth, const C* __restrict__ color, size_t px,
+                                             float* __restrict__ out_depth, C* __restrict__ out_color) {
+  *out_depth = depth[px];
+  out_color[0] = color[3 * px]; out_color[1] = color[3 * px + 1]; out_color[2] = color[3 * px + 2];
+}
+struct TrackSampleArgs {
+  const float* cam; const int64_t* draws; int n;
+  const float* depth; const double* color; int W, H0, W0, Wr;
+  float fx, fy, cx, cy; Bound6 B;
+  float* rays_o; float* rays_d; float* dirs; float* gt_depth; double* gt_color; int32_t* kept_index; int32_t* count;
+};
+__global__ void __launch_bounds__(1024) track_sample_kernel(const __grid_constant__ TrackSampleArgs A) {
+  __shared__ float m[12];
+  __shared__ int warp_tot[32];
+  __shared__ int carry;
+  if (threadIdx.x == 0) { cam_to_c2w(A.cam, m); carry = 0; }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int base = 0; base < A.n; base += blockDim.x) {
+    const int r = base + threadIdx.x;
+    float o[3], d[3], dir[3], gd = 0.0f;
+    size_t px = 0;
+    bool keep = false;
+    if (r < A.n) {
+      const long long k = A.draws[r];
+      const int i = A.W0 + (int)(k % A.Wr), j = A.H0 + (int)(k / A.Wr);
+      pixel_ray(m, (float)i, (float)j, A.fx, A.fy, A.cx, A.cy, o, d, dir);
+      px = (size_t)j * A.W + i;
+      gd = A.depth[px];
+      keep = bbox_keep(A.B.b, o, d, gd);
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) warp_tot[warp] = __popc(b);
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      int t = threadIdx.x < (blockDim.x >> 5) ? warp_tot[threadIdx.x] : 0;
+      for (int s = 1; s < 32; s <<= 1) { const int u = __shfl_up_sync(0xffffffffu, t, s); if (lane >= s) t += u; }
+      warp_tot[threadIdx.x] = t;                                   // inclusive over warps
+    }
+    __syncthreads();
+    if (keep) {
+      const int p = carry + (warp ? warp_tot[warp - 1] : 0) + __popc(b & ((1u << lane) - 1u));
+#pragma unroll
+      for (int a = 0; a < 3; a++) { A.rays_o[3 * p + a] = o[a]; A.rays_d[3 * p + a] = d[a]; A.dirs[3 * p + a] = dir[a]; }
+      gather_pixel(A.depth, A.color, px, A.gt_depth + p, A.gt_color + 3 * p);
+      if (A.kept_index != nullptr) A.kept_index[p] = r;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) carry += warp_tot[31];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) A.count[0] = carry;
+}
+// Tracker pose step, one thread: the iteration's loss joins losses[iter] and the best-pose bookkeeping (Tracker.py:223-247: strict `<` against the
+// running minimum, which starts at 1e10 -- the caller's best[0]); d c2w (float64, the fused backward's sum) is rounded to float32, where the
+// reference's autograd chain runs, chained through quad2rotation and Adam steps the camera tensor.  The candidate is the camera tensor the loss
+// was evaluated at (post_step = 0) or the one after this step (post_step = 1); c2w16 = its pose as a [4][4] with the [0,0,0,1] row.
+__global__ void track_pose_step_kernel(float* __restrict__ cam, const double* __restrict__ loss, const double* __restrict__ d_c2w,
+                                       float* __restrict__ em, float* __restrict__ ev, const AdamScalars aq, const AdamScalars at, int iter, int post_step,
+                                       double* __restrict__ losses, double* __restrict__ best, float* __restrict__ candidate, float* __restrict__ c2w16) {
+  if (threadIdx.x != 0) return;
+  const double L = loss[0];
+  losses[iter] = L;
+  const bool better = L < best[0];                                  // false for NaN
+  if (better) {
+    best[0] = L; best[1] = (double)iter;
+    if (!post_step) for (int t = 0; t < 7; t++) candidate[t] = cam[t];
+  }
+  float g[12];
+  for (int t = 0; t < 12; t++) g[t] = (float)d_c2w[t];
+  pose_adam_step(cam, g, em, ev, nullptr, aq, at);
+  if (better) {
+    if (post_step) for (int t = 0; t < 7; t++) candidate[t] = cam[t];
+    float m[12];
+    cam_to_c2w(candidate, m);
+    for (int t = 0; t < 12; t++) c2w16[t] = m[t];
+    c2w16[12] = 0.0f; c2w16[13] = 0.0f; c2w16[14] = 0.0f; c2w16[15] = 1.0f;
   }
 }
 extern "C" int nsb_window_rays(const float* cams, const int32_t* cam_row, const float* fixed_c2w, int n_frames,
@@ -758,6 +856,31 @@ extern "C" int nsb_adam_poses(float* cams, const int32_t* cam_row, int n_frames,
   AdamScalars a; int rc = adam_scalars(lr, beta1, beta2, eps, step, &a); if (rc) return rc;
   adam_poses_kernel<<<(n_frames + 63) / 64, 64, 0, (cudaStream_t)stream>>>(cams, cam_row, n_frames, d_c2w, exp_avg, exp_avg_sq, d_cams, a);
   return check_cuda(cudaGetLastError(), "adam_poses launch");
+}
+extern "C" int nsb_track_samples(const float* cam, const int64_t* draws, int n, const float* depth, const double* color, int H, int W,
+                                 int H0, int H1, int W0, int W1, double fx, double fy, double cx, double cy, const double bound[6],
+                                 float* rays_o, float* rays_d, float* dirs, float* gt_depth, double* gt_color, int32_t* kept_index,
+                                 int32_t* count, void* stream) {
+  if (!cam || !depth || !color || !bound || !count || n < 0 || (n > 0 && (!draws || !rays_o || !rays_d || !dirs || !gt_depth || !gt_color)) ||
+      H < 1 || W < 1 || H0 < 0 || H0 >= H1 || H1 > H || W0 < 0 || W0 >= W1 || W1 > W) {
+    set_error("track_samples: bad arguments"); return NSB_ERR_ARG; }
+  TrackSampleArgs A;
+  A.cam = cam; A.draws = draws; A.n = n; A.depth = depth; A.color = color; A.W = W; A.H0 = H0; A.W0 = W0; A.Wr = W1 - W0;
+  A.fx = (float)fx; A.fy = (float)fy; A.cx = (float)cx; A.cy = (float)cy;
+  for (int i = 0; i < 6; i++) A.B.b[i] = bound[i];
+  A.rays_o = rays_o; A.rays_d = rays_d; A.dirs = dirs; A.gt_depth = gt_depth; A.gt_color = gt_color; A.kept_index = kept_index; A.count = count;
+  track_sample_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(A);
+  return check_cuda(cudaGetLastError(), "track_samples launch");
+}
+extern "C" int nsb_track_pose_step(float* cam, const double* loss, const double* d_c2w, float* exp_avg, float* exp_avg_sq, double lr, double quat_lr,
+                                   double beta1, double beta2, double eps, int step, int post_step, double* losses, double* best,
+                                   float* candidate, float* c2w16, void* stream) {
+  if (!cam || !loss || !d_c2w || !exp_avg || !exp_avg_sq || !losses || !best || !candidate || !c2w16) { set_error("track_pose_step: bad arguments"); return NSB_ERR_ARG; }
+  AdamScalars at, aq; int rc;
+  if ((rc = adam_scalars(lr, beta1, beta2, eps, step, &at)) || (rc = adam_scalars(quat_lr, beta1, beta2, eps, step, &aq))) return rc;
+  track_pose_step_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(cam, loss, d_c2w, exp_avg, exp_avg_sq, aq, at, step - 1, post_step ? 1 : 0,
+                                                              losses, best, candidate, c2w16);
+  return check_cuda(cudaGetLastError(), "track_pose_step launch");
 }
 
 extern "C" size_t nsb_frustum_mask_workspace(long long n_voxels) { return n_voxels <= 0 ? 16 : (size_t)n_voxels * sizeof(float) + 16; }
@@ -909,9 +1032,7 @@ __global__ void keyframe_gather_kernel(const float* __restrict__ depth, const fl
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n_frames * n_pix) return;
   const int f = idx / n_pix;
-  const size_t px = ((size_t)slot[f] * H + pix_j[idx]) * W + pix_i[idx];
-  out_depth[idx] = depth[px];
-  out_color[3 * idx] = color[3 * px]; out_color[3 * idx + 1] = color[3 * px + 1]; out_color[3 * idx + 2] = color[3 * px + 2];
+  gather_pixel(depth, color, ((size_t)slot[f] * H + pix_j[idx]) * W + pix_i[idx], out_depth + idx, out_color + 3 * idx);
 }
 extern "C" int nsb_keyframe_gather(const float* depth, const float* color, const int32_t* slot, const int32_t* pix_i, const int32_t* pix_j,
                                    int n_frames, int n_pix, int H, int W, float* out_depth, float* out_color, void* stream) {
