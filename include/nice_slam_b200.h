@@ -97,7 +97,9 @@ int nsb_debug_occupancy(int* fwd_ctas_per_sm, int* bwd_ctas_per_sm);
 int nsb_pack_decoders(const nsb_decoder_params* const params[4], float* const packed[4], void* stream);
 
 /* Batch-global depth maxima used by the sampler: out[0] = max(gt_depth), out[1] = max(gt_depth*1.2f)
- * (src/utils/Renderer.py:109,144).  n may be 0 (out := 0). */
+ * (src/utils/Renderer.py:109,144).  n may be 0 (out := 0).  A NaN sensor depth is skipped (the maxima are those of the other rays;
+ * -inf if every depth is NaN), where torch.max would return NaN and the reference's sampler would then make every sample of the
+ * batch NaN; the reductions inside the render kernels (depth_max == NULL, gt_depth_batch) do the same. */
 int nsb_batch_max_depth(const float* gt_depth, int n, float* out2, void* stream);
 
 /* Ray pre-filter (src/Tracker.py:95-104, src/Mapper.py:471-481): keep[i] = (t_exit(ray i) >= gt_depth[i]). */

@@ -167,7 +167,8 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
   __syncthreads();
   if (handle_dynamic) {
     // torch.median = lower median = the element of rank (n-1)/2 of the IEEE bit patterns (residuals are non-negative, so the unsigned
-    // 64-bit pattern is order preserving; NaN sorts last like torch.sort).
+    // 64-bit pattern is order preserving).  torch.median of a pool that holds a NaN IS NaN -- the mask r < 10 * NaN then keeps no ray and
+    // the loss is 0 --, so the loops that read the pool also look for one and the selected key is replaced by NaN at the end.
     const double* mp = pool != nullptr ? pool : res;       // sharded batches: median over the all-gathered residuals
     int np = pool != nullptr ? n_pool : n;
     int pool_pitch = 0;                                    // > 0: the pool is [world][pool_pitch] with n valid entries per rank
@@ -191,11 +192,12 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
     }
     auto pool_at = [&](int i) { return pool_pitch ? mp[(size_t)(i / n) * pool_pitch + (i % n)] : mp[i]; };
     const int k = (np - 1) / 2;
+    int saw_nan = 0, pool_nan = 0;                         // this thread met a NaN in the pool / some thread did (CTA-uniform)
     // the key of rank `want` among keys[0 .. cnt), cnt <= kMedianDirect: direct rank counting from shared memory (no serial passes) or a sort
     auto select_direct = [&](int cnt, int want) {
       if (cnt > 256) {
         // more than one key per thread: bitonic sort in shared memory (45 compare-exchange stages for 512 keys) beats cnt^2 / 256 comparisons.
-        // Padding with ~0 sorts behind every key (NaN patterns included), so the key of rank `want` is simply keys[want].
+        // Padding with ~0 sorts behind every key, so the key of rank `want` is simply keys[want].
         int m = 512;                                             // == kMedianDirect (capacity of keys[])
         for (int i = cnt + threadIdx.x; i < m; i += blockDim.x) keys[i] = ~0ull;
         __syncthreads();
@@ -222,8 +224,12 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
     };
     if (np <= kMedianDirect) {
       // small pools (a tracking batch is 200 rays)
-      for (int i = threadIdx.x; i < np; i += blockDim.x) keys[i] = (unsigned long long)__double_as_longlong(pool_at(i));
-      __syncthreads();
+      for (int i = threadIdx.x; i < np; i += blockDim.x) {
+        const double v = pool_at(i);
+        saw_nan |= v != v;
+        keys[i] = (unsigned long long)__double_as_longlong(v);
+      }
+      pool_nan = __syncthreads_or(saw_nan);
       select_direct(np, k);
     } else {
       // radix select, 8 bits per pass over a 256-bin shared histogram -- until the bin that holds the wanted rank is small enough for the direct
@@ -236,10 +242,12 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
         __syncthreads();
         const unsigned long long maskhi = shift == 56 ? 0ull : (~0ull << (shift + 8));
         for (int i = threadIdx.x; i < np; i += blockDim.x) {
-          const unsigned long long key = (unsigned long long)__double_as_longlong(pool_at(i));
+          const double v = pool_at(i);
+          saw_nan |= v != v;
+          const unsigned long long key = (unsigned long long)__double_as_longlong(v);
           if ((key & maskhi) == prefix) atomicAdd(&hist[(int)((key >> shift) & 0xffull)], 1);
         }
-        __syncthreads();
+        pool_nan = __syncthreads_or(saw_nan);              // (every pass reads the whole pool)
         // digit of the k-th key = the bin whose [exclusive, inclusive) prefix-count range contains kk (256 bins: 8 warps scan them)
         {
           const int v = threadIdx.x < 256 ? hist[threadIdx.x] : 0;
@@ -276,7 +284,7 @@ __device__ __forceinline__ void tracking_seeds_body(const double* depth, const d
         __syncthreads();
       }
     }
-    if (threadIdx.x == 0) med_s = __longlong_as_double((long long)med_key);
+    if (threadIdx.x == 0) med_s = pool_nan ? __longlong_as_double(0x7ff8000000000000ll) : __longlong_as_double((long long)med_key);
     __syncthreads();
   }
   double acc = 0.0;

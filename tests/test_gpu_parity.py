@@ -211,72 +211,6 @@ def test_eval_points_matches_oracle():
         assert torch.equal(got[:, 3].cpu() == 100, want[:, 3] == 100)
 
 
-@pytest.mark.parametrize("n", [777, 200, 5000])      # radix-select median (> 512 residuals), direct rank counting, radix again
-def test_seed_kernels_match_reference_losses(n):
-    import ctypes as C
-    from nice_slam_b200 import _lib
-    L = _lib.lib()
-    g = torch.Generator().manual_seed(9)
-    depth = torch.rand(n, generator=g, dtype=torch.float64) * 3
-    var = torch.rand(n, generator=g, dtype=torch.float64) * 0.1
-    rgb = torch.rand(n, 3, generator=g)
-    gt = torch.rand(n, generator=g) * 3
-    gt[::13] = 0
-    gt_rgb = torch.rand(n, 3, generator=g, dtype=torch.float64)
-    # tracking
-    d1 = depth.clone().requires_grad_(True); c1 = rgb.clone().requires_grad_(True)
-    loss = tp.tracking_loss(d1, var, c1, gt, gt_rgb, 0.5)
-    loss.backward()
-    dev = lambda t: t.to(DEV)
-    gD = torch.empty(n, dtype=torch.float64, device=DEV); gC = torch.empty(n, 3, device=DEV); lo = torch.empty(1, dtype=torch.float64, device=DEV)
-    ws = torch.empty(L.nsb_tracking_seeds_workspace(n), dtype=torch.uint8, device=DEV)
-    t = [dev(depth), dev(var), dev(rgb), dev(gt), dev(gt_rgb)]
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _lib.check(L.nsb_tracking_seeds(*[C.c_void_p(x.data_ptr()) for x in t], n, 0.5, 1, 1, None, 0, C.c_void_p(gD.data_ptr()), C.c_void_p(gC.data_ptr()),
-                                    C.c_void_p(lo.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), st), "tracking_seeds")
-    assert abs(float(lo) - float(loss)) < 1e-9 * abs(float(loss))
-    assert rel(gD, d1.grad) < 1e-12 and rel(gC, c1.grad) < 1e-6
-    # median over an external pool (the all-gathered residuals of a sharded batch): mask = r < 10 * median(pool)
-    pool = torch.rand(1601, generator=g, dtype=torch.float64) * 2.0
-    res = torch.abs(gt.double() - depth) / torch.sqrt(var + 1e-10)
-    m = (res < 10 * pool.median()) & (gt > 0)
-    want = res[m].sum() + 0.5 * torch.abs(gt_rgb - rgb.double())[m].sum()
-    pool_d = dev(pool)
-    _lib.check(L.nsb_tracking_seeds(*[C.c_void_p(x.data_ptr()) for x in t], n, 0.5, 1, 1, C.c_void_p(pool_d.data_ptr()), pool.numel(),
-                                    C.c_void_p(gD.data_ptr()), C.c_void_p(gC.data_ptr()), C.c_void_p(lo.data_ptr()), C.c_void_p(ws.data_ptr()),
-                                    ws.numel(), st), "tracking_seeds(pool)")
-    assert float(want) > 0 and abs(float(lo) - float(want)) < 1e-9 * abs(float(want))
-    # mapping
-    d2 = depth.clone().requires_grad_(True); c2 = rgb.clone().requires_grad_(True)
-    loss2 = tp.mapping_loss(d2, c2, gt, gt_rgb.float(), "color", 0.2)
-    loss2.backward()
-    t2 = [dev(depth), dev(rgb), dev(gt), dev(gt_rgb.float())]
-    _lib.check(L.nsb_mapping_seeds(*[C.c_void_p(x.data_ptr()) for x in t2], n, 0.2, 1, C.c_void_p(gD.data_ptr()), C.c_void_p(gC.data_ptr()),
-                                   C.c_void_p(lo.data_ptr()), st), "mapping_seeds")
-    assert abs(float(lo) - float(loss2)) < 1e-6 * abs(float(loss2))
-    assert rel(gD, d2.grad) < 1e-12 and rel(gC, c2.grad) < 1e-6
-
-
-def test_prefilter_and_batch_max():
-    import ctypes as C
-    from nice_slam_b200 import _lib
-    L = _lib.lib()
-    sc = su.load_scenes()["room0"]
-    bound = su.scene_bound(sc)
-    ro, rd, gd, _ = su.make_rays(sc, 5000, seed=1)
-    keep = tp.bbox_prefilter(ro, rd, gd, bound)
-    k = torch.empty(5000, dtype=torch.uint8, device=DEV)
-    b6 = (C.c_double * 6)(*bound.reshape(6).tolist())
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    ro_d, rd_d, gd_d = ro.to(DEV), rd.to(DEV), gd.to(DEV)
-    _lib.check(L.nsb_bbox_prefilter(C.c_void_p(ro_d.data_ptr()), C.c_void_p(rd_d.data_ptr()), C.c_void_p(gd_d.data_ptr()), 5000, b6,
-                                    C.c_void_p(k.data_ptr()), st), "prefilter")
-    assert torch.equal(k.cpu().bool(), keep)
-    out = torch.empty(2, device=DEV)
-    _lib.check(L.nsb_batch_max_depth(C.c_void_p(gd_d.data_ptr()), 5000, C.c_void_p(out.data_ptr()), st), "batch_max")
-    assert float(out[0]) == float(torch.max(gd)) and float(out[1]) == float(torch.max(gd * 1.2))
-
-
 # ------------------------------------------------------------------------------------ edge cases & properties
 @pytest.mark.parametrize("n_samples,n_surface,n_rays", [(5, 3, 37), (4, 2, 29), (32, 16, 1), (16, 16, 333), (80, 16, 50), (32, 0, 64)])
 def test_ragged_shapes_against_oracle(n_samples, n_surface, n_rays):
