@@ -353,6 +353,21 @@ int nsb_track_pose_step(float* cam, const double* loss, const double* d_c2w, flo
                         double beta1, double beta2, double eps, int step, int post_step, double* losses, double* best,
                         float* candidate, float* c2w16, void* stream);
 
+/* ---- the mapper's window sampler (src/Mapper.py:426-481: per-row get_samples, torch.cat, bbox pre-filter) ----------------------------------
+ * nsb_map_samples (one launch per joint iteration): a window of n_rows (1..NSB_MAP_MAX_ROWS) rows, each with n_per_row flat draws of the full
+ * H x W image (int64, draws[f * n_per_row + r]; draw k is pixel i = k % W, j = k / W, get_sample_uv(0, H, 0, W, ...)).  Row f reads the images
+ * of keyframe-store slot slot[f] (depth [slots][H][W], colour [slots][H][W][3], float32) and is posed as in nsb_window_rays (camera tensor
+ * cams[cam_row[f]], or fixed_c2w[f] where cam_row[f] < 0; cams may be NULL when every row is fixed).  Each ray is computed as get_rays_from_uv
+ * does and kept if the bbox pre-filter of nsb_bbox_prefilter keeps it.  Kept rays go compacted in draw order (what boolean indexing of the
+ * concatenated batch gives) to rays_o, rays_d, dirs, gt_depth, gt_color [capacity n_rows * n_per_row]; frame_offsets [n_rows + 1] = kept rays
+ * before each row (nsb_pose_grad_frames' input); count[0] = rays kept.  Draws must lie in [0, H*W). */
+#define NSB_MAP_MAX_ROWS 64
+int nsb_map_samples(const int64_t* draws, int n_rows, int n_per_row, const int32_t* slot, const float* depth, const float* color,
+                    int H, int W, const float* cams, const int32_t* cam_row, const float* fixed_c2w,
+                    double fx, double fy, double cx, double cy, const double bound[6],
+                    float* rays_o, float* rays_d, float* dirs, float* gt_depth, float* gt_color, int32_t* frame_offsets,
+                    int32_t* count, void* stream);
+
 /* ---- exchanges of a ray-sharded tracking iteration through NVLink peer memory (SURVEY.md 8e) ---------------------------------
  * A batch sharded over `world` GPUs (equal shards) needs three batch-global quantities: max(gt_depth) (Renderer.py:109,144), the
  * median of the residuals (Tracker.py:113) and the sums of loss and pose gradient.  The *_peers variants of the three single-CTA

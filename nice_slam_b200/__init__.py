@@ -3,10 +3,12 @@
 Public surface:
     FusedRenderer   mirror of the reference's Renderer (render_batch_ray / eval_points / render_img)
     NICEDecoders    parameter container with the reference's state_dict keys
+    FusedMapper     one Mapper.optimize_map call on the fused path (mapping.py)
     to_channels_last, lib (ctypes handle of libnsb.so)
 """
 from ._lib import lib, LIB_PATH                       # noqa: F401
 from .decoders import NICEDecoders                     # noqa: F401
 from .renderer import FusedRenderer, to_channels_last  # noqa: F401
+from .mapping import FusedMapper                       # noqa: F401
 
-__all__ = ["FusedRenderer", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH"]
+__all__ = ["FusedRenderer", "FusedMapper", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH"]

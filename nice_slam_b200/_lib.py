@@ -130,6 +130,8 @@ SYMBOLS = {
     "nsb_adam_poses": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _P]),
     "nsb_track_samples": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
                                     C.c_double, C.c_double, C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
+    "nsb_map_samples": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_double, C.c_double, C.c_double,
+                                  C.c_double, C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
     "nsb_track_pose_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int,
                                       _P, _P, _P, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),

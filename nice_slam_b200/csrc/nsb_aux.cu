@@ -1,5 +1,6 @@
 // nsb_aux.cu -- small kernels on either side of the render kernels + library plumbing:
 //   decoder packing / gradient unpacking, batch depth maxima, ray pre-filter, loss seeds.
+#include <climits>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -689,14 +690,18 @@ __device__ __forceinline__ void cam_to_c2w(const float* __restrict__ cam, float*
   m[10] = __fsub_rn(1.0f, __fmul_rn(s, __fadd_rn(__fmul_rn(qi, qi), __fmul_rn(qj, qj))));
   m[3] = cam[4]; m[7] = cam[5]; m[11] = cam[6];
 }
-// poses of the window rows: row f uses camera tensor cam_row[f] (>= 0) or, for the fixed oldest frame (-1), fixed_c2w[f]
+// pose of window row f: camera tensor cam_row[f] (>= 0) or, for a fixed row (-1), fixed_c2w[f]
+__device__ __forceinline__ void window_pose(const float* __restrict__ cams, const int32_t* __restrict__ cam_row, const float* __restrict__ fixed_c2w,
+                                            int f, float* __restrict__ m) {
+  if (cam_row[f] >= 0) cam_to_c2w(cams + 7 * cam_row[f], m);
+  else for (int k = 0; k < 12; k++) m[k] = fixed_c2w[12 * f + k];
+}
 __global__ void window_poses_kernel(const float* __restrict__ cams, const int32_t* __restrict__ cam_row, const float* __restrict__ fixed_c2w,
                                     int n_frames, float* __restrict__ c2w_out) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n_frames) return;
   float m[12];
-  if (cam_row[f] >= 0) cam_to_c2w(cams + 7 * cam_row[f], m);
-  else for (int k = 0; k < 12; k++) m[k] = fixed_c2w[12 * f + k];
+  window_pose(cams, cam_row, fixed_c2w, f, m);
   for (int k = 0; k < 12; k++) c2w_out[12 * f + k] = m[k];
 }
 // get_rays_from_uv (src/common.py:74-89): dirs = [(i-cx)/fx, -(j-cy)/fy, -1]; rays_d = sum_j dirs_j * R[:, j]; rays_o = t
@@ -766,31 +771,35 @@ __device__ __forceinline__ void gather_pixel(const float* __restrict__ depth, co
   *out_depth = depth[px];
   out_color[0] = color[3 * px]; out_color[1] = color[3 * px + 1]; out_color[2] = color[3 * px + 2];
 }
-struct TrackSampleArgs {
-  const float* cam; const int64_t* draws; int n;
-  const float* depth; const double* color; int W, H0, W0, Wr;
-  float fx, fy, cx, cy; Bound6 B;
-  float* rays_o; float* rays_d; float* dirs; float* gt_depth; double* gt_color; int32_t* kept_index; int32_t* count;
-};
-__global__ void __launch_bounds__(1024) track_sample_kernel(const __grid_constant__ TrackSampleArgs A) {
-  __shared__ float m[12];
+// Where the draws of one sampler row look: its pose m [3][4] and its depth / colour image.
+template <typename C> struct SampleRow { const float* m; const float* depth; const C* color; };
+template <typename C> struct SampleOut { float* rays_o; float* rays_d; float* dirs; float* gt_depth; C* gt_color; int32_t* kept_index; int32_t* frame_offsets; };
+// The loop both samplers run, one CTA of up to 1024 threads: draw r belongs to row r / n_per_row (row_of(row) -> SampleRow); its flat index k
+// is pixel i = W0 + k % Wr, j = H0 + k / Wr of that row's W-wide image -> ray (pixel_ray) -> sensor depth -> bbox pre-filter.  Kept rays are
+// compacted in draw order by a ballot / warp-scan per round of blockDim.x draws.  frame_offsets (optional) [n / n_per_row + 1]: kept rays
+// before each row boundary (what nsb_pose_grad_frames takes).  Returns the kept count (valid in thread 0).
+template <typename C, typename RowOf>
+__device__ __forceinline__ int sample_compact(const int64_t* __restrict__ draws, int n, int n_per_row, int W, int H0, int W0, int Wr,
+                                              float fx, float fy, float cx, float cy, const Bound6& B, const RowOf& row_of, const SampleOut<C>& out) {
   __shared__ int warp_tot[32];
   __shared__ int carry;
-  if (threadIdx.x == 0) { cam_to_c2w(A.cam, m); carry = 0; }
+  if (threadIdx.x == 0) { carry = 0; if (out.frame_offsets != nullptr) out.frame_offsets[0] = 0; }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int base = 0; base < A.n; base += blockDim.x) {
+  for (int base = 0; base < n; base += blockDim.x) {
     const int r = base + threadIdx.x;
     float o[3], d[3], dir[3], gd = 0.0f;
     size_t px = 0;
     bool keep = false;
-    if (r < A.n) {
-      const long long k = A.draws[r];
-      const int i = A.W0 + (int)(k % A.Wr), j = A.H0 + (int)(k / A.Wr);
-      pixel_ray(m, (float)i, (float)j, A.fx, A.fy, A.cx, A.cy, o, d, dir);
-      px = (size_t)j * A.W + i;
-      gd = A.depth[px];
-      keep = bbox_keep(A.B.b, o, d, gd);
+    SampleRow<C> row{};
+    if (r < n) {
+      row = row_of(r / n_per_row);
+      const long long k = draws[r];
+      const int i = W0 + (int)(k % Wr), j = H0 + (int)(k / Wr);
+      pixel_ray(row.m, (float)i, (float)j, fx, fy, cx, cy, o, d, dir);
+      px = (size_t)j * W + i;
+      gd = row.depth[px];
+      keep = bbox_keep(B.b, o, d, gd);
     }
     const unsigned b = __ballot_sync(0xffffffffu, keep);
     if (lane == 0) warp_tot[warp] = __popc(b);
@@ -801,18 +810,64 @@ __global__ void __launch_bounds__(1024) track_sample_kernel(const __grid_constan
       warp_tot[threadIdx.x] = t;                                   // inclusive over warps
     }
     __syncthreads();
+    const int p = carry + (warp ? warp_tot[warp - 1] : 0) + __popc(b & ((1u << lane) - 1u));
     if (keep) {
-      const int p = carry + (warp ? warp_tot[warp - 1] : 0) + __popc(b & ((1u << lane) - 1u));
 #pragma unroll
-      for (int a = 0; a < 3; a++) { A.rays_o[3 * p + a] = o[a]; A.rays_d[3 * p + a] = d[a]; A.dirs[3 * p + a] = dir[a]; }
-      gather_pixel(A.depth, A.color, px, A.gt_depth + p, A.gt_color + 3 * p);
-      if (A.kept_index != nullptr) A.kept_index[p] = r;
+      for (int a = 0; a < 3; a++) { out.rays_o[3 * p + a] = o[a]; out.rays_d[3 * p + a] = d[a]; out.dirs[3 * p + a] = dir[a]; }
+      gather_pixel(row.depth, row.color, px, out.gt_depth + p, out.gt_color + 3 * p);
+      if (out.kept_index != nullptr) out.kept_index[p] = r;
     }
+    if (out.frame_offsets != nullptr && r < n && (r + 1) % n_per_row == 0) out.frame_offsets[(r + 1) / n_per_row] = p + (keep ? 1 : 0);
     __syncthreads();
     if (threadIdx.x == 0) carry += warp_tot[31];
     __syncthreads();
   }
-  if (threadIdx.x == 0) A.count[0] = carry;
+  return carry;
+}
+struct TrackSampleArgs {
+  const float* cam; const int64_t* draws; int n;
+  const float* depth; const double* color; int W, H0, W0, Wr;
+  float fx, fy, cx, cy; Bound6 B;
+  float* rays_o; float* rays_d; float* dirs; float* gt_depth; double* gt_color; int32_t* kept_index; int32_t* count;
+};
+struct OneFrame {
+  const float* m; const float* depth; const double* color;
+  __device__ SampleRow<double> operator()(int) const { return {m, depth, color}; }
+};
+__global__ void __launch_bounds__(1024) track_sample_kernel(const __grid_constant__ TrackSampleArgs A) {
+  __shared__ float m[12];
+  if (threadIdx.x == 0) cam_to_c2w(A.cam, m);
+  __syncthreads();
+  const SampleOut<double> out{A.rays_o, A.rays_d, A.dirs, A.gt_depth, A.gt_color, A.kept_index, nullptr};
+  const int kept = sample_compact(A.draws, A.n, A.n > 0 ? A.n : 1, A.W, A.H0, A.W0, A.Wr, A.fx, A.fy, A.cx, A.cy, A.B, OneFrame{m, A.depth, A.color}, out);
+  if (threadIdx.x == 0) A.count[0] = kept;
+}
+
+// ---- the mapper's window sampler (Mapper.optimize_map's per-row get_samples + torch.cat + bbox pre-filter, src/Mapper.py:426-481) -----------
+// One CTA: row f of the window is keyframe-store slot slot[f] under the pose window_pose(f) (camera tensor or fixed); draws of the full image.
+struct MapSampleArgs {
+  const int64_t* draws; int n_rows, n_per_row;
+  const int32_t* slot; const float* depth; const float* color; int H, W;
+  const float* cams; const int32_t* cam_row; const float* fixed_c2w;
+  float fx, fy, cx, cy; Bound6 B;
+  float* rays_o; float* rays_d; float* dirs; float* gt_depth; float* gt_color; int32_t* frame_offsets; int32_t* count;
+};
+struct WindowRows {
+  const float* m; const size_t* image; const float* depth; const float* color;     // m [rows][12] and image offsets in shared memory
+  __device__ SampleRow<float> operator()(int f) const { return {m + 12 * f, depth + image[f], color + 3 * image[f]}; }
+};
+__global__ void __launch_bounds__(1024) map_sample_kernel(const __grid_constant__ MapSampleArgs A) {
+  __shared__ float m[NSB_MAP_MAX_ROWS * 12];
+  __shared__ size_t image[NSB_MAP_MAX_ROWS];
+  if (threadIdx.x < A.n_rows) {
+    window_pose(A.cams, A.cam_row, A.fixed_c2w, threadIdx.x, m + 12 * threadIdx.x);
+    image[threadIdx.x] = (size_t)A.slot[threadIdx.x] * A.H * A.W;
+  }
+  __syncthreads();
+  const SampleOut<float> out{A.rays_o, A.rays_d, A.dirs, A.gt_depth, A.gt_color, nullptr, A.frame_offsets};
+  const int kept = sample_compact(A.draws, A.n_rows * A.n_per_row, A.n_per_row, A.W, 0, 0, A.W, A.fx, A.fy, A.cx, A.cy, A.B,
+                                  WindowRows{m, image, A.depth, A.color}, out);
+  if (threadIdx.x == 0) A.count[0] = kept;
 }
 // Tracker pose step, one thread: the iteration's loss joins losses[iter] and the best-pose bookkeeping (Tracker.py:223-247: strict `<` against the
 // running minimum, which starts at 1e10 -- the caller's best[0]); d c2w (float64, the fused backward's sum) is rounded to float32, where the
@@ -871,6 +926,25 @@ extern "C" int nsb_track_samples(const float* cam, const int64_t* draws, int n, 
   A.rays_o = rays_o; A.rays_d = rays_d; A.dirs = dirs; A.gt_depth = gt_depth; A.gt_color = gt_color; A.kept_index = kept_index; A.count = count;
   track_sample_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(A);
   return check_cuda(cudaGetLastError(), "track_samples launch");
+}
+extern "C" int nsb_map_samples(const int64_t* draws, int n_rows, int n_per_row, const int32_t* slot, const float* depth, const float* color,
+                               int H, int W, const float* cams, const int32_t* cam_row, const float* fixed_c2w,
+                               double fx, double fy, double cx, double cy, const double bound[6],
+                               float* rays_o, float* rays_d, float* dirs, float* gt_depth, float* gt_color, int32_t* frame_offsets,
+                               int32_t* count, void* stream) {
+  if (n_rows < 1 || n_rows > NSB_MAP_MAX_ROWS || n_per_row < 1 || (long long)n_rows * n_per_row > INT_MAX) {
+    set_error("map_samples: %d rows x %d draws (1..%d rows, >= 1 draw each)", n_rows, n_per_row, NSB_MAP_MAX_ROWS); return NSB_ERR_ARG; }
+  if (!draws || !slot || !depth || !color || H < 1 || W < 1 || !cam_row || (!cams && !fixed_c2w) || !bound ||
+      !rays_o || !rays_d || !dirs || !gt_depth || !gt_color || !frame_offsets || !count) {
+    set_error("map_samples: bad arguments"); return NSB_ERR_ARG; }
+  MapSampleArgs A;
+  A.draws = draws; A.n_rows = n_rows; A.n_per_row = n_per_row; A.slot = slot; A.depth = depth; A.color = color; A.H = H; A.W = W;
+  A.cams = cams; A.cam_row = cam_row; A.fixed_c2w = fixed_c2w;
+  A.fx = (float)fx; A.fy = (float)fy; A.cx = (float)cx; A.cy = (float)cy;
+  for (int i = 0; i < 6; i++) A.B.b[i] = bound[i];
+  A.rays_o = rays_o; A.rays_d = rays_d; A.dirs = dirs; A.gt_depth = gt_depth; A.gt_color = gt_color; A.frame_offsets = frame_offsets; A.count = count;
+  map_sample_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(A);
+  return check_cuda(cudaGetLastError(), "map_samples launch");
 }
 extern "C" int nsb_track_pose_step(float* cam, const double* loss, const double* d_c2w, float* exp_avg, float* exp_avg_sq, double lr, double quat_lr,
                                    double beta1, double beta2, double eps, int step, int post_step, double* losses, double* best,

@@ -16,6 +16,14 @@ from . import _lib
 from .renderer import _VP, _stream
 
 
+def pick_overlap(counts, n_points, k, rng=np.random):
+    """The selection policy of Mapper.keyframe_selection_overlap (Mapper.py:218-227) on per-keyframe overlap counts of n_points points:
+    keyframes with percent_inside > 0, sorted by it (stable, descending), permuted with numpy's RNG, first k."""
+    lst = sorted([{"id": i, "percent_inside": c / n_points} for i, c in enumerate(counts)], key=lambda d: d["percent_inside"], reverse=True)
+    sel = [d["id"] for d in lst if d["percent_inside"] > 0.00]
+    return list(rng.permutation(np.array(sel))[:k])
+
+
 class KeyframeStore:
     def __init__(self, H, W, fx, fy, cx, cy, device, capacity=16):
         self.H, self.W, self.fx, self.fy, self.cx, self.cy = int(H), int(W), float(fx), float(fy), float(cx), float(cy)
@@ -82,10 +90,17 @@ class KeyframeStore:
         """Mapper.keyframe_selection_overlap (src/Mapper.py:166-228) given the caller's pixel draw (get_samples, torch RNG): ids of up to k
         keyframes with overlap, sorted by percent_inside (stable, descending), permuted with numpy's RNG, as the reference does."""
         counts = self.overlap_counts(rays_o, rays_d, gt_depth, n_samples, n_keyframes=n_keyframes).cpu().numpy()
-        n = int(rays_o.shape[0]) * int(n_samples)
-        lst = sorted([{"id": i, "percent_inside": c / n} for i, c in enumerate(counts)], key=lambda d: d["percent_inside"], reverse=True)
-        sel = [d["id"] for d in lst if d["percent_inside"] > 0.00]
-        return list(rng.permutation(np.array(sel))[:k])
+        return pick_overlap(counts, int(rays_o.shape[0]) * int(n_samples), k, rng)
+
+    def stage(self, gt_color, gt_depth):
+        """Copy a frame's images into the first free slot without registering it as a keyframe (the mapper's current frame, which it samples
+        like a keyframe).  Returns the slot; the next append() overwrites it."""
+        k = len(self.idx)
+        if k == self._cap:
+            self._grow(2 * self._cap)
+        self.depth[k].copy_(torch.as_tensor(gt_depth).to(self.dev, torch.float32))
+        self.color[k].copy_(torch.as_tensor(gt_color).to(self.dev, torch.float32))
+        return k
 
     def sample(self, slots, pix_i, pix_j):
         """gt_depth [F,n] and gt_color [F,n,3] (float32, device) of pixels (pix_i, pix_j) ([F,n] integer tensors, the caller's get_sample_uv draws)

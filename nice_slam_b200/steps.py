@@ -120,17 +120,7 @@ class IterationContext:
         self.gt_color = self.d_in[col_off:].view(col_dt).view(n, 3)
         self.grad_grids = tuple(grad_grids)
         self.grad_decoders = tuple(grad_decoders)
-        self.masked = dict(masked or {})
-        self.n_frames = int(n_frames)
-        # packed float32 gradient block = what a sharded mapping iteration all-reduces in ONE collective (SURVEY.md 8e):
-        #   [loss, 0, 0, 0 | d c2w of the keyframes (12 each) | decoder grads (canonical flat order) | compact voxel grads]
-        # every section starts on a 16-byte boundary (the voxel scatter uses 16-byte vector reductions)
-        sect, off = packed_layout(self.n_frames, self.grad_decoders, [(k, self.masked[k].count) for k in self.grad_grids if k in self.masked])
-        self.sections = sect
-        self.packed = torch.zeros(off, dtype=f32, device=dev)
-        self.d_frames = self.packed[4: 4 + 12 * self.n_frames].view(self.n_frames, 12)
-        self.d_grid = {key: self.packed[sect[key][0]: sect[key][0] + sect[key][1]].view(-1, 32) for key in self.grad_grids if key in self.masked}
-        self.d_flat = {lvl: self.packed[sect["dec_" + lvl][0]: sect["dec_" + lvl][0] + sect["dec_" + lvl][1]] for lvl in self.grad_decoders}
+        self.rebind(masked, n_frames)
         # layer outputs of the fine / colour decoders, kept by the forward when their weight gradients are wanted: the backward then computes them
         # on the tensor cores (nsb_forward_outputs.acts / acts_levels); 640 B per sample point and decoder.  A set with the middle or coarse
         # decoder takes the FP32-FMA pass, which reads no acts, unless the library option wgrad_all is on (then every decoder's are kept).
@@ -152,6 +142,22 @@ class IterationContext:
         self.h_pose13 = torch.empty(13, dtype=f64).pin_memory() if cuda else None
         self.h2d_bytes = self.d_in.numel()
         self.d2h_bytes = self.d_res.numel()
+
+    def rebind(self, masked, n_frames):
+        """(Re)build the packed gradient block for a voxel selection `masked` and a window of n_frames keyframes, keeping every ray-sized
+        buffer: a mapper reuses one context per stage across frames, whose frustum selections differ."""
+        self.masked = dict(masked or {})
+        self.n_frames = int(n_frames)
+        # packed float32 gradient block = what a sharded mapping iteration all-reduces in ONE collective (SURVEY.md 8e):
+        #   [loss, 0, 0, 0 | d c2w of the keyframes (12 each) | decoder grads (canonical flat order) | compact voxel grads]
+        # every section starts on a 16-byte boundary (the voxel scatter uses 16-byte vector reductions)
+        sect, off = packed_layout(self.n_frames, self.grad_decoders, [(k, self.masked[k].count) for k in self.grad_grids if k in self.masked])
+        self.sections = sect
+        self.packed = torch.zeros(off, dtype=torch.float32, device=self.dev)
+        self.d_frames = self.packed[4: 4 + 12 * self.n_frames].view(self.n_frames, 12)
+        self.d_grid = {key: self.packed[sect[key][0]: sect[key][0] + sect[key][1]].view(-1, 32) for key in self.grad_grids if key in self.masked}
+        self.d_flat = {lvl: self.packed[sect["dec_" + lvl][0]: sect["dec_" + lvl][0] + sect["dec_" + lvl][1]] for lvl in self.grad_decoders}
+        return self
 
     # ------------------------------------------------------------------------------------------
     def _grads(self, c):
