@@ -197,11 +197,12 @@ def random_select(l, k, rng=np.random):
 class FusedMapper:
     def __init__(self, renderer, c, decoders, store, pixels=1000, mapping_window_size=5, middle_iter_ratio=0.4, fine_iter_ratio=0.6, stage=None,
                  BA_cam_lr=0.001, w_color_loss=0.2, keyframe_selection_method="overlap", fix_fine=True, fix_color=False,
-                 frustum_feature_selection=True, coarse_mapper=False):
+                 frustum_feature_selection=True, coarse_mapper=False, generator=None, rng=None):
         """renderer / c / decoders: the mapper's renderer, shared grids (updated in place) and decoders; store: the keyframes
         (keyframes.KeyframeStore, device-resident images).  The other arguments are cfg['mapping'] settings under the reference's names
         (`stage` is the per-stage learning-rate dict); the coarse mapper always selects keyframes globally (Mapper.py:78-80) and optimises
-        grid_coarse only."""
+        grid_coarse only.  generator / rng: the torch.Generator (on the grids' device) of the pixel draws and the numpy RandomState of the
+        keyframe selection; None takes torch's default generator and numpy's global state."""
         require_default_sampling(renderer, "FusedMapper")
         if stage is None:
             raise RuntimeError("FusedMapper: the per-stage learning rates (cfg['mapping']['stage']) are required")
@@ -210,6 +211,7 @@ class FusedMapper:
         self.middle_iter_ratio, self.fine_iter_ratio = float(middle_iter_ratio), float(fine_iter_ratio)
         self.stage_cfg, self.BA_cam_lr, self.w_color_loss = stage, float(BA_cam_lr), float(w_color_loss)
         self.coarse_mapper = bool(coarse_mapper)
+        self.generator, self.rng = generator, (np.random if rng is None else rng)
         self.keyframe_selection_method = "global" if self.coarse_mapper else keyframe_selection_method
         self.fix_fine, self.fix_color, self.frustum_feature_selection = bool(fix_fine), bool(fix_color), bool(frustum_feature_selection)
         self.keys = ("grid_coarse",) if self.coarse_mapper else ("grid_middle", "grid_fine", "grid_color")
@@ -231,11 +233,11 @@ class FusedMapper:
         if K == 0:
             return []
         if self.keyframe_selection_method == "global":
-            return random_select(K - 1, self.window_size - 2)
+            return random_select(K - 1, self.window_size - 2, self.rng)
         if self.keyframe_selection_method != "overlap":
             raise RuntimeError("FusedMapper: unknown keyframe_selection_method %r" % self.keyframe_selection_method)
         H, W = self.store.H, self.store.W
-        k = torch.randint(H * W, (100,), device=self.dev)         # keyframe_selection_overlap's get_samples(0, H, 0, W, 100, ...)
+        k = torch.randint(H * W, (100,), device=self.dev, generator=self.generator)       # keyframe_selection_overlap's get_samples(0, H, 0, W, 100, ...)
         pi, pj = (k % W).float(), (k // W).float()
         fixed = cur_c2w.to(self.dev, torch.float32)[:3, :4].reshape(1, 12).contiguous()
         cam_row = torch.full((1,), -1, dtype=torch.int32, device=self.dev)
@@ -245,13 +247,13 @@ class FusedMapper:
                                               _VP(frame.data_ptr()), 100, float(self.r.fx), float(self.r.fy), float(self.r.cx), float(self.r.cy),
                                               _VP(c2w.data_ptr()), _VP(ro.data_ptr()), _VP(rd.data_ptr()), None, _stream()), "nsb_window_rays")
         gd, _ = self.store.sample([slot_cur], pi.view(1, -1), pj.view(1, -1))
-        return self.store.select_overlap(ro, rd, gd.view(-1), self.window_size - 2, n_keyframes=K - 1)
+        return self.store.select_overlap(ro, rd, gd.view(-1), self.window_size - 2, n_keyframes=K - 1, rng=self.rng)
 
     def map_frame(self, num_joint_iters, lr_factor, cur_gt_color, cur_gt_depth, cur_c2w, ba, draws=None, selection=None):
         """One Mapper.optimize_map call (src/Mapper.py:230-540) for the current frame (cur_gt_color [H,W,3], cur_gt_depth [H,W], estimated pose
         cur_c2w [4,4]) against the keyframes of the store.  ba: bundle adjustment (the reference's self.BA).  draws: optional
         [num_joint_iters, F, pixs_per_image] flat pixel indices (k = j * W + i) of every window row; without it each iteration calls
-        torch.randint(H*W, (pixs_per_image,)) once per row in row order, as the reference's get_samples does.  selection: optional keyframe
+        torch.randint(H*W, (pixs_per_image,)) once per row in row order (from self.generator), as the reference's get_samples does.  selection: optional keyframe
         ids replacing the keyframe selection (and its random draws).  Afterwards self.losses holds the per-iteration losses (device float64),
         self.window the window's keyframe ids (-1: the current frame), self.fixed_row its fixed row and self.stages the stage schedule.
         Returns the optimised current pose [4,4] (device float32) with bundle adjustment, else None; the optimised keyframe poses are
@@ -301,7 +303,7 @@ class FusedMapper:
                 d = draws[it]
             else:
                 for f in range(F):                                 # the reference's per-row get_samples draws, in row order
-                    torch.randint(H * W, (ppi,), out=draw_buf[f])
+                    torch.randint(H * W, (ppi,), out=draw_buf[f], generator=self.generator)
                 d = draw_buf
             _lib.check(L.nsb_map_samples(_VP(d.data_ptr()), F, ppi, _VP(slots.data_ptr()), _VP(store.depth.data_ptr()), _VP(store.color.data_ptr()),
                                          H, W, _VP(cams.data_ptr()) if cams is not None else None, _VP(cam_row.data_ptr()), _VP(fixed.data_ptr()),

@@ -18,10 +18,11 @@ BETAS, EPS = (0.9, 0.999), 1e-8                 # torch.optim.Adam defaults (Tra
 
 class FusedTrackingLoop:
     def __init__(self, renderer, c, decoders, capacity, ignore_edge_W=20, ignore_edge_H=20, pixels=None, iters=10, lr=0.001,
-                 seperate_LR=False, handle_dynamic=True, use_color_in_tracking=True, w_color_loss=0.5, const_speed_assumption=True):
+                 seperate_LR=False, handle_dynamic=True, use_color_in_tracking=True, w_color_loss=0.5, const_speed_assumption=True,
+                 generator=None):
         """c / decoders: the tracker's grids and decoders (read only); capacity: rays per iteration the buffers are sized for
         (cfg['tracking']['pixels']).  The other arguments are cfg['tracking'] settings under the reference's names; pixels defaults to
-        capacity."""
+        capacity.  generator: the torch.Generator (on the grids' device) the pixel draws come from; None draws from torch's default one."""
         require_default_sampling(renderer, "FusedTrackingLoop")
         self.r, self.c, self.dec, self.capacity = renderer, c, decoders, int(capacity)
         self.pixels = self.capacity if pixels is None else int(pixels)
@@ -30,6 +31,7 @@ class FusedTrackingLoop:
         self.ignore_edge_W, self.ignore_edge_H, self.iters, self.lr = int(ignore_edge_W), int(ignore_edge_H), int(iters), float(lr)
         self.seperate_LR, self.handle_dynamic, self.use_color = bool(seperate_LR), bool(handle_dynamic), bool(use_color_in_tracking)
         self.w_color_loss, self.const_speed_assumption = float(w_color_loss), bool(const_speed_assumption)
+        self.generator = generator
         H, W = int(renderer.H), int(renderer.W)
         self.H0, self.H1, self.W0, self.W1 = self.ignore_edge_H, H - self.ignore_edge_H, self.ignore_edge_W, W - self.ignore_edge_W
         if self.iters < 1 or self.H0 < 0 or self.W0 < 0 or self.H1 <= self.H0 or self.W1 <= self.W0:
@@ -68,7 +70,8 @@ class FusedTrackingLoop:
         """Optimise the camera of one frame for `iters` iterations and return the chosen pose, [4,4] float32 on the device (Tracker.py:248-253).
         gt_color [H,W,3], gt_depth [H,W]: the frame (copied to the device once).  init_c2w: the start pose ([4,4] or [3,4], converted by
         mapping.tensor_from_c2w on the host, as the reference's get_tensor_from_camera does) or a camera tensor [7] [qw,qx,qy,qz,tx,ty,tz].  draws: optional [iters, pixels] flat indices into the
-        edge-cropped region; without it every iteration draws torch.randint(n_region, (pixels,)) on the frame's device, as select_uv does.
+        edge-cropped region; without it every iteration draws torch.randint(n_region, (pixels,)) on the frame's device (from self.generator),
+        as select_uv does.
         Afterwards self.losses holds the per-iteration losses (device float64) and self.best_iter the chosen iteration."""
         L = _lib.lib()
         st = _stream()
@@ -90,7 +93,8 @@ class FusedTrackingLoop:
         post_step = 0 if self.seperate_LR else 1
         quat_lr = self.lr * 0.2 if self.seperate_LR else self.lr
         for it in range(self.iters):
-            n = self.sample(draws[it] if draws is not None else torch.randint(self.n_region, (self.pixels,), device=self.dev))
+            n = self.sample(draws[it] if draws is not None else torch.randint(self.n_region, (self.pixels,), device=self.dev,
+                                                                                         generator=self.generator))
             if n == 0:
                 raise RuntimeError("FusedTrackingLoop: the bbox pre-filter kept no ray in iteration %d (the reference fails in median())" % it)
             self.iterate(n)
