@@ -399,6 +399,76 @@ int nsb_pose_grad_peers(const float* dirs, const float* d_rays_o, const float* d
 /* Points-only decode (Renderer.eval_points, src/utils/Renderer.py:23-61): p f64 [P,3] -> raw f32 [P,4]. */
 int nsb_eval_points(const nsb_render_inputs* in, const double* points, int n_points, float* raw, void* stream);
 
+/* ---- mesh extraction (Mesher.get_mesh, src/utils/Mesher.py:349-574; nsb_mesh.cu) ------------------------------------------------------------
+ * Differences from the reference, by design:
+ *  - the scene hull is the convex hull of the keyframes' camera centres and back-projected depth pixels (nsb_mesh_hull_*), not of the
+ *    vertices of open3d's TSDF surface (voxel 4 scale/512, truncation 0.04 scale; Mesher.py:214-279), which lie within about a voxel of them;
+ *  - marching cubes uses the case table of tools/gen_mc_table.py (nsb_mc_table.h): the same vertex set as skimage's, but in cells with an
+ *    ambiguous face the triangles may differ from its Lewiner variant;
+ *  - the lattice and colour decodes normalise the float32 points to the bound in float64 (Mesher.eval_points does it in float32): the
+ *    occupancies agree to the eval_points tolerances, the in-bound decision is the reference's float32 one. */
+
+/* Marching-cubes lattice of get_grid_uniform (Mesher.py:321-347): axis a has n[a] values np.linspace(start, stop, n) = start + i * step,
+ * the last one stop (all float64, as numpy computes them); point (ix, iy, iz) = float32 of the three values. */
+typedef struct {
+  int32_t n[3];
+  double start[3], step[3], stop[3];
+  const double* planes;          /* device f64 [n_planes][4] half-spaces of the scene hull, n . p + d <= 0 inside; NULL = no hull */
+  int32_t n_planes;
+} nsb_mesh_lattice;
+
+/* Mesher.eval_points at stage 'fine' over the lattice + the hull test (Mesher.py:281-319, 421-433): z f32 [nx, ny, nz] = occupancy logit
+ * (channel 3), 100 where the float32 point is not strictly inside the float32-rounded in->bound or lies outside the hull (:315, :433).
+ * The decode is nsb_eval_points' tile forward (a mesh instantiation of the same kernel body) with the points generated in the kernel; it
+ * needs the tile kernels (mlp_backend 0 or 3: NSB_ERR_UNSUPPORTED otherwise); in->stage must be NSB_STAGE_FINE. */
+int nsb_mesh_lattice_eval(const nsb_render_inputs* in, const nsb_mesh_lattice* lat, float* z, void* stream);
+
+/* direct_point_query (Mesher.py:513-524, 555-556): vertices f64 [V,3] rounded to float32, decoded at stage 'color' (in->stage) with the
+ * float32 in-bound rule; colors u8 [V,3] = uint8(clip(rgb, 0, 1) * 255) (truncating).  raw: scratch f32 [V,4]. */
+int nsb_mesh_colors(const nsb_render_inputs* in, const double* vertices, int n_vertices, float* raw, uint8_t* colors, void* stream);
+
+/* Marching cubes over z f32 [nx,ny,nz] (replaces skimage.measure.marching_cubes, Mesher.py:437-467).  A corner is inside iff z > level;
+ * one vertex per crossed lattice edge, shared by every cell on that edge, ordered by (lattice point, axis); vertex of the edge from point
+ * p along axis a at ((p + t e_a) * spacing + origin) in float64, t = (level - z(p)) / (z(p + e_a) - z(p)); faces in (cell, table) order,
+ * wound so that their normals point from inside (occupied) to outside (free) corners.  Two calls: nsb_mc_count (per-point counts and
+ * their exclusive scan into the workspace; totals[0] = vertices, totals[1] = faces, device int64) then nsb_mc_emit with outputs of that size.
+ * edge_ids (optional, int64 [V]): a * nx*ny*nz + linear(p) of each vertex's lattice edge. */
+size_t nsb_mc_workspace(long long n_points);
+int nsb_mc_count(const float* z, const int32_t n[3], double level, void* workspace, size_t workspace_bytes, long long* totals, void* stream);
+int nsb_mc_emit(const float* z, const int32_t n[3], double level, const double origin[3], const double spacing[3], const void* workspace,
+                double* vertices, int32_t* faces, long long* edge_ids, void* stream);
+
+/* Scene-hull candidates (replaces get_bound_from_frames' TSDF, Mesher.py:214-279).  Every pixel with depth > 0 of the M frames
+ * depth f32 [M][H][W] is back-projected with c2w f64 [M][3][4]: x = (u - cx)/fx d, y = -(v - cy)/fy d, z = -d.  nsb_mesh_hull_support:
+ * best u64 [K] (zero it first) = max over the pixels of (order-preserving bits of float32(dir_k . p)) << 32 | pixel index, for the K
+ * directions dirs f64 [K][3].  nsb_mesh_hull_outside: the pixels with  n . p + d > -tol  for any of the inner polytope's half-spaces
+ * planes f64 [P][4] -> flag u8 [M*H*W] (1 = survivor; 0 also for depth <= 0).  nsb_mesh_hull_points: world point f64 [3] of pixel ids. */
+int nsb_mesh_hull_support(const float* depth, int M, int H, int W, const double* c2w, double fx, double fy, double cx, double cy,
+                          const double* dirs, int K, unsigned long long* best, void* stream);
+int nsb_mesh_hull_outside(const float* depth, int M, int H, int W, const double* c2w, double fx, double fy, double cx, double cy,
+                          const double* planes, int n_planes, double tol, uint8_t* flag, void* stream);
+int nsb_mesh_hull_points(const float* depth, int H, int W, const double* c2w, double fx, double fy, double cx, double cy,
+                         const long long* ids, int n, double* points, void* stream);
+
+/* point_masks' seen output (Mesher.py:53-212, depth_test False), one launch for V vertices x M poses, in the reference's float32 order:
+ * p = float32(vertex); cam = w2c [p, 1] (w2c f32 [M][16] = float32(inv(c2w)) computed in float64); cam.x = -cam.x; uv = K cam;
+ * z = uv.z + 1e-8f; seen |= 0 < uv.x/z < W && 0 < uv.y/z < H && z < 0 && (depth_limit == NULL || -cam.z < depth_limit[m]).
+ * nsb_mesh_depth_limits: depth_limit[m] = max(depth[m]) * 1.1f (keyframe mode, :179). */
+int nsb_mesh_depth_limits(const float* depth, int M, long long hw, float* depth_limit, void* stream);
+int nsb_mesh_seen(const double* vertices, int n_vertices, const float* w2c, int M, const float* depth_limit, double fx, double fy,
+                  double cx, double cy, int H, int W, uint8_t* seen, void* stream);
+
+/* Culling, shared-edge components and compaction (Mesher.py:469-511): a face is dropped iff its three vertices are unseen; faces sharing
+ * an edge (an unordered vertex pair) are connected; component areas are float64 sums of the face areas (atomic: their order, and so the
+ * last bit, may vary between calls); components with area > threshold are kept, or with largest != 0 only the largest.  nsb_mesh_clean:
+ * totals[0] = kept vertices, totals[1] = kept faces (device int64); nsb_mesh_compact writes them, vertices in their old order, faces
+ * re-indexed. */
+size_t nsb_mesh_clean_workspace(int n_vertices, int n_faces);
+int nsb_mesh_clean(const double* vertices, int n_vertices, const int32_t* faces, int n_faces, const uint8_t* seen, double threshold,
+                   int largest, void* workspace, size_t workspace_bytes, long long* totals, void* stream);
+int nsb_mesh_compact(const double* vertices, int n_vertices, const int32_t* faces, int n_faces, const void* workspace,
+                     double* out_vertices, int32_t* out_faces, void* stream);
+
 /* Pose-gradient reduction: rays_d = sum_j dirs_j * R[:,j], rays_o = t (get_rays_from_uv, src/common.py:74-89) =>
  * d c2w[i][j] = sum_r d_rays_d[r][i] * dirs[r][j] (j<3), d c2w[i][3] = sum_r d_rays_o[r][i].  dirs: [N,3] camera-frame
  * directions.  d_c2w: float64 [3][4], OVERWRITTEN.  The quaternion chain (quad2rotation, src/common.py:137-160) stays in

@@ -70,6 +70,11 @@ class IterationBuffers(C.Structure):
                 ("event_bwd_begin", C.c_void_p), ("event_bwd_end", C.c_void_p), ("acts", C.c_void_p), ("acts_levels", C.c_int)]
 
 
+class MeshLattice(C.Structure):
+    _fields_ = [("n", C.c_int32 * 3), ("start", C.c_double * 3), ("step", C.c_double * 3), ("stop", C.c_double * 3),
+                ("planes", C.c_void_p), ("n_planes", C.c_int32)]
+
+
 class Peers(C.Structure):
     _fields_ = [("rank", C.c_int), ("world", C.c_int), ("buffer", C.c_void_p * 8), ("counters", C.c_void_p), ("max_rays", C.c_int)]
 
@@ -134,6 +139,20 @@ SYMBOLS = {
                                   C.c_double, C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
     "nsb_track_pose_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int,
                                       _P, _P, _P, _P, _P]),
+    "nsb_mesh_lattice_eval": (C.c_int, [C.POINTER(RenderInputs), C.POINTER(MeshLattice), _P, _P]),
+    "nsb_mesh_colors": (C.c_int, [C.POINTER(RenderInputs), _P, C.c_int, _P, _P, _P]),
+    "nsb_mc_workspace": (C.c_size_t, [C.c_longlong]),
+    "nsb_mc_count": (C.c_int, [_P, C.POINTER(C.c_int32), C.c_double, _P, C.c_size_t, _P, _P]),
+    "nsb_mc_emit": (C.c_int, [_P, C.POINTER(C.c_int32), C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double), _P, _P, _P, _P, _P]),
+    "nsb_mesh_hull_support": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, C.c_int, _P, _P]),
+    "nsb_mesh_hull_outside": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, C.c_int,
+                                        C.c_double, _P, _P]),
+    "nsb_mesh_hull_points": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, C.c_int, _P, _P]),
+    "nsb_mesh_depth_limits": (C.c_int, [_P, C.c_int, C.c_longlong, _P, _P]),
+    "nsb_mesh_seen": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, _P, _P]),
+    "nsb_mesh_clean_workspace": (C.c_size_t, [C.c_int, C.c_int]),
+    "nsb_mesh_clean": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, C.c_size_t, _P, _P]),
+    "nsb_mesh_compact": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),
     "nsb_batch_max_depth_peers": (C.c_int, [_P, C.c_int, _P, C.POINTER(Peers), _P]),
     "nsb_tracking_seeds_peers": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(Peers), _P, _P, _P, _P, C.c_size_t, _P]),

@@ -217,6 +217,10 @@ int render_forward_fused(const nsb_render_inputs* in, const nsb_forward_outputs*
 int render_backward_tail(const nsb_render_inputs* in, const nsb_backward_args* bw, const PeerTail* tail, void* stream, bool after_forward = false,
                          const nsb_sampling* smp = nullptr);
 int make_peerx(const struct nsb_peers* p, PeerX* px);
+// nsb_eval_points' tile forward for mesh extraction, with the points rounded to float32 and Mesher.eval_points' float32 in-bound rule:
+// points f64 [n,3] -> raw f32 [n,4], or (points NULL) the mesh lattice `lat` and its hull -> z f32 [n]
+int eval_points_mesh(const nsb_render_inputs* in, const double* points, const nsb_mesh_lattice* lat, int n_points, float* raw, float* z,
+                     void* stream);
 
 // error plumbing shared by the API translation units
 void set_error(const char* fmt, ...);

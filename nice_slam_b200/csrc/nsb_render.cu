@@ -172,6 +172,36 @@ struct KParams {
   nsb_sampling smp;             // lindisp / perturb uniforms / a given sorted z list (all zero: the default sampler)
 };
 
+// Mesh extraction (nsb_mesh.cu) runs the points-mode tile forward with this second parameter block (the other kernels do not carry it):
+// the points are P.points rounded to float32, or (lattice != 0) the lattice points (ix, iy, iz) = float32 of np.linspace's values
+// (Mesher.get_grid_uniform, Mesher.py:334-345); the in-bound test is Mesher.eval_points' float32 one (Mesher.py:301-304), and a point
+// outside the hull's half-spaces counts as out of bound (z = 100, Mesher.py:433); lattice occupancies go to z [P] instead of raw.
+struct MeshPoints { nsb_mesh_lattice lat; int lattice; float* z; };
+__device__ __forceinline__ double lattice_value(const nsb_mesh_lattice& L, int a, int i) {
+  return i == L.n[a] - 1 ? L.stop[a] : __dadd_rn(__dmul_rn((double)i, L.step[a]), L.start[a]);
+}
+__device__ __forceinline__ void mesh_point_geom(const KParams& P, const MeshPoints& M, long long gp, PointGeom& G) {
+  double pin[3];
+  if (M.lattice) {
+    const long long nyz = (long long)M.lat.n[1] * M.lat.n[2];
+    const int ix = (int)(gp / nyz), iy = (int)((gp - ix * nyz) / M.lat.n[2]), iz = (int)(gp - ix * nyz - (long long)iy * M.lat.n[2]);
+    pin[0] = lattice_value(M.lat, 0, ix); pin[1] = lattice_value(M.lat, 1, iy); pin[2] = lattice_value(M.lat, 2, iz);
+  } else {
+    pin[0] = P.points[3 * gp]; pin[1] = P.points[3 * gp + 1]; pin[2] = P.points[3 * gp + 2];
+  }
+  for (int a = 0; a < 3; a++) pin[a] = (double)(float)pin[a];
+  make_point_from_p(P.in.bound, P.in.coarse_bound, pin, G);
+  G.inb = 1;
+  for (int a = 0; a < 3; a++) {
+    const float p = (float)pin[a];
+    if (!(p < (float)P.in.bound[2 * a + 1] && p > (float)P.in.bound[2 * a])) G.inb = 0;
+  }
+  for (int k = 0; k < M.lat.n_planes && G.inb; k++) {
+    const double* h = M.lat.planes + 4 * k;
+    if (__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(h[0], pin[0]), __dmul_rn(h[1], pin[1])), __dmul_rn(h[2], pin[2])), h[3]) > 0.0) G.inb = 0;
+  }
+}
+
 struct Smem {                   // carve-up of dynamic shared memory (all offsets 16-byte aligned)
   float* wt; uint64_t* bar; float* rays; double* far; double* zs; float* raw; double* dp; float* gocc; float* wgt;
   unsigned char* inb; float* act;
@@ -1267,6 +1297,7 @@ static int set_attrs() {
     {(const void*)render_fwd_tile_kernel, tile_smem_bytes(false), true, "render_fwd_tile_kernel"},
     {(const void*)render_fwd_tile_h16_kernel, tile_smem_bytes(false), true, "render_fwd_tile_h16_kernel"},
     {(const void*)render_fwd_tile_sampled_kernel, tile_smem_bytes(false), true, "render_fwd_tile_sampled_kernel"},
+    {(const void*)render_fwd_tile_mesh_kernel, tile_smem_bytes(false), true, "render_fwd_tile_mesh_kernel"},
     {(const void*)render_bwd_tile_kernel, tile_smem_bytes(true), true, "render_bwd_tile_kernel"},
     {(const void*)render_bwd_wg_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_tile_kernel"},
     {(const void*)render_bwd_wg_coarse_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_coarse_tile_kernel"},
@@ -1383,6 +1414,21 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
   }
   if (fam == Family::Group) return launch_group(K, false, out->split_workspace, out->split_workspace_bytes, (cudaStream_t)stream);
   return launch_fma(K, false, (cudaStream_t)stream);
+}
+
+// nsb_eval_points' tile forward for mesh extraction: float32 points (the caller's, or the lattice `lat`) and the float32 in-bound rule
+int nsb::eval_points_mesh(const nsb_render_inputs* in, const double* points, const nsb_mesh_lattice* lat, int n_points, float* raw, float* z,
+                          void* stream) {
+  int rc = validate_inputs(in, false); if (rc) return rc;
+  if (n_points == 0) return NSB_OK;
+  if (kernel_family(1, 0, true) != Family::Tile) { set_error("mesh extraction runs on the tile kernels (mlp_backend 0 or 3)"); return NSB_ERR_UNSUPPORTED; }
+  KParams K; fill_common(K, in); memset(&K.fo, 0, sizeof(K.fo)); memset(&K.bw, 0, sizeof(K.bw));
+  K.points = points; K.points_raw = raw; K.n_points = n_points; K.S = 1; K.has_gt = 0;
+  MeshPoints M; memset(&M, 0, sizeof(M));
+  if (lat != nullptr) { M.lat = *lat; M.lattice = 1; M.z = z; }
+  if ((rc = set_attrs())) return rc;
+  render_fwd_tile_mesh_kernel<<<(unsigned)tile_count(n_points), tl::kThreads, tile_smem_bytes(false), (cudaStream_t)stream>>>(K, M);
+  return check_cuda(cudaGetLastError(), "render_fwd_tile_mesh_kernel launch");
 }
 
 extern "C" int nsb_eval_points(const nsb_render_inputs* in, const double* points, int n_points, float* raw, void* stream) {

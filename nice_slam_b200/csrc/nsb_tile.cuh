@@ -1133,8 +1133,8 @@ __device__ __forceinline__ void composite_ray(const KParams& P, int ray, int lan
 // ================================================================================================================================
 // forward kernel
 // ================================================================================================================================
-template <bool H16, bool kSampled = false>
-__device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
+template <bool H16, bool kSampled = false, bool kMesh = false>
+__device__ __forceinline__ void render_fwd_tile_body(const KParams& P, const MeshPoints* M = nullptr) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using namespace tl;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1144,7 +1144,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   __shared__ float s_max[16];
   __shared__ uint32_t s_seq;
 
-  const bool points = P.points != nullptr;
+  const bool points = kMesh || P.points != nullptr;
   const int nsplit = P.split;
   const int tile = blockIdx.x / nsplit, my = blockIdx.x - tile * nsplit;
   const int q0 = nsplit > 1 ? my : 0, q1 = nsplit > 1 ? my + 1 : P.n_dec;
@@ -1172,8 +1172,12 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   const int lp = row < npts ? row : npts - 1;
   if (points) {
     const long long gp = gp0 + lp;
-    const double pin[3] = {P.points[3 * gp], P.points[3 * gp + 1], P.points[3 * gp + 2]};
-    make_point_from_p(P.in.bound, P.in.coarse_bound, pin, G);
+    if constexpr (kMesh) {
+      mesh_point_geom(P, *M, gp, G);
+    } else {
+      const double pin[3] = {P.points[3 * gp], P.points[3 * gp + 1], P.points[3 * gp + 2]};
+      make_point_from_p(P.in.bound, P.in.coarse_bound, pin, G);
+    }
     __syncthreads();
   } else {
     float gtmax, gtmax12;
@@ -1233,7 +1237,10 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P) {
   NSB_PH(14);
 
   if (points) {                                                   // Renderer.eval_points: raw with the out-of-bound override
-    if (cg == 0 && row < npts) *reinterpret_cast<float4*>(P.points_raw + 4 * (gp0 + row)) = make_float4(c0, c1, c2, G.inb ? occ : 100.0f);
+    if (cg == 0 && row < npts) {
+      if (kMesh && M->z != nullptr) M->z[gp0 + row] = G.inb ? occ : 100.0f;
+      else *reinterpret_cast<float4*>(P.points_raw + 4 * (gp0 + row)) = make_float4(c0, c1, c2, G.inb ? occ : 100.0f);
+    }
     return;
   }
   if (cg == 0 && row < npts) P.tile_parts[(long long)my * NP + gp0 + row] = make_float4(c0, c1, c2, occ);
@@ -1248,6 +1255,10 @@ __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_kernel(const 
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_h16_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<true>(P); }
 // lindisp / perturb / a given sample list (KParams::smp, nsb_render_forward_sampled)
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_sampled_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false, true>(P); }
+// mesh extraction's points (MeshPoints): the 3xTF32 forward
+__global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_mesh_kernel(const __grid_constant__ KParams P, const __grid_constant__ MeshPoints M) {
+  render_fwd_tile_body<false, false, true>(P, &M);
+}
 
 // ================================================================================================================================
 // backward kernel (input gradients: rays + grid voxels)

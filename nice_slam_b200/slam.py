@@ -3,6 +3,7 @@
 same time.  Per frame: tracking.FusedTrackingLoop.track_frame; every `every_frame` frames and on the last one: mapping.FusedMapper.map_frame
 (and the coarse mapper's).  Checkpoints follow the reference's Logger.log, so its eval_ate.py, mesher and visualiser read a fused run."""
 import os
+import shutil
 import time
 
 import numpy as np
@@ -10,6 +11,7 @@ import torch
 
 from .keyframes import KeyframeStore
 from .mapping import FusedMapper
+from .mesh import FusedMesher
 from .tracking import FusedTrackingLoop
 
 MAPPER_KEYS = ("pixels", "mapping_window_size", "middle_iter_ratio", "fine_iter_ratio", "stage", "BA_cam_lr", "w_color_loss",
@@ -37,15 +39,24 @@ class FusedSLAM:
       grid_coarse, so that choice cannot move a pose.
 
     Each component draws from its own torch.Generator on the device and its own numpy RandomState, seeded from `seed` (self.seeds), as the
-    reference's three processes each have their own random state."""
+    reference's three processes each have their own random state.
 
-    def __init__(self, renderer, c, decoders, cfg, seed=0, ckpt_dir=None):
+    With mesh_dir, the fine mapper's frames are meshed as Mapper.py:636-653 meshes them (mesh.FusedMesher, after the checkpoint):
+    {idx:05d}_mesh.ply when idx % mesh_freq == 0 (not frame 0 under no_mesh_on_first_frame); on the last frame final_mesh.ply and a copy
+    as {idx:05d}_mesh.ply, and with meshing.eval_rec final_mesh_eval_rec.ply culled with every frame's pose.  The scene hull is the
+    convex hull of the keyframes' depth points rather than of open3d's TSDF surface (see mesh.py).  Meshing reads the grids only and
+    draws no random numbers; its wall time goes to times['meshing']."""
+
+    def __init__(self, renderer, c, decoders, cfg, seed=0, ckpt_dir=None, mesh_dir=None):
         """renderer / c / decoders: a FusedRenderer, the shared grids (updated in place) and decoders; cfg: the reference's loaded config
-        (cfg['tracking'], cfg['mapping'], cfg['coarse'], cfg['sync_method']).  ckpt_dir: where the checkpoints go (none without it)."""
+        (cfg['tracking'], cfg['mapping'], cfg['coarse'], cfg['sync_method']; with mesh_dir also cfg['meshing'], cfg['scale'] and
+        mapping.marching_cubes_bound / mesh_freq / no_mesh_on_first_frame).  ckpt_dir: where the checkpoints go (none without it);
+        mesh_dir: where the meshes go (no meshing without it)."""
         if cfg["sync_method"] != "strict":
             raise RuntimeError("FusedSLAM: sync_method %r is not supported; only 'strict' gives a result that does not depend on timing"
                                % cfg["sync_method"])
-        self.r, self.c, self.dec, self.cfg, self.ckpt_dir = renderer, c, decoders, cfg, ckpt_dir
+        self.r, self.c, self.dec, self.cfg, self.ckpt_dir, self.mesh_dir = renderer, c, decoders, cfg, ckpt_dir, mesh_dir
+        self.mesher = FusedMesher(renderer, cfg) if mesh_dir is not None else None
         mp = cfg["mapping"]
         self.every_frame, self.keyframe_every, self.ckpt_freq = int(mp["every_frame"]), int(mp["keyframe_every"]), int(mp["ckpt_freq"])
         self.color_refine, self.no_log_on_first_frame = bool(mp["color_refine"]), bool(mp["no_log_on_first_frame"])
@@ -54,7 +65,7 @@ class FusedSLAM:
         self.gt_camera = bool(cfg["tracking"]["gt_camera"])
         self.seeds = {"tracker": int(seed), "mapper": int(seed) + 1, "coarse": int(seed) + 2}
         self.dev = next(iter(c.values())).device
-        self.run_log, self.times = [], dict.fromkeys(PHASES, 0.0)
+        self.run_log, self.times = [], self._phases()
         self.estimate_c2w_list = self.gt_c2w_list = None
         self._build()
 
@@ -105,7 +116,7 @@ class FusedSLAM:
         self.estimate_c2w_list = torch.zeros(n, 4, 4)
         self.gt_c2w_list = torch.zeros(n, 4, 4)
         self.selected_keyframes = {} if self.save_selected else None
-        self.run_log, self.times = [], dict.fromkeys(PHASES, 0.0)
+        self.run_log, self.times = [], self._phases()
         self._replay = {k: list(replay.get(k, ())) for k in ("map", "coarse")}
         self._replay_track = replay.get("track", {})
         H, W = int(self.r.H), int(self.r.W)
@@ -128,6 +139,9 @@ class FusedSLAM:
                 if idx % self.every_frame == 0 or idx == n - 1:
                     self._map_frame(idx, color, depth, gt_c2w)
         return self.estimate_c2w_list.clone(), self.gt_c2w_list.clone()
+
+    def _phases(self):
+        return dict.fromkeys(PHASES + (("meshing",) if self.mesher is not None else ()), 0.0)
 
     def _timed(self, phase, t0):
         if self.dev.type == "cuda":
@@ -185,6 +199,24 @@ class FusedSLAM:
             t0 = time.perf_counter()
             self.log(idx)
             self._timed("checkpoints", t0)
+        if self.mesher is not None:
+            t0 = time.perf_counter()
+            self._mesh(idx)
+            self._timed("meshing", t0)
+
+    def _mesh(self, idx):
+        """Mapper.py:636-653 with the fine mapper's keyframes and estimate_c2w_list."""
+        mp, ms = self.cfg["mapping"], self.cfg["meshing"]
+        clean = bool(ms.get("clean_mesh", True))
+        state = (self.c, self.dec, self.store, self.estimate_c2w_list, idx)
+        if idx % int(mp["mesh_freq"]) == 0 and not (idx == 0 and mp["no_mesh_on_first_frame"]):
+            self.mesher.get_mesh(os.path.join(self.mesh_dir, "{:05d}_mesh.ply".format(idx)), *state, clean_mesh=clean)
+        if idx == self.n_img - 1:
+            final = os.path.join(self.mesh_dir, "final_mesh.ply")
+            if self.mesher.get_mesh(final, *state, clean_mesh=clean) is not None:
+                shutil.copyfile(final, os.path.join(self.mesh_dir, "{:05d}_mesh.ply".format(idx)))
+            if ms.get("eval_rec"):
+                self.mesher.get_mesh(os.path.join(self.mesh_dir, "final_mesh_eval_rec.ply"), *state, clean_mesh=clean, get_mask_use_all_frames=True)
 
     def _call(self, mapper, kind, idx, iters, lr_factor, color, depth, cur, gt_c2w, ba, refine):
         """One optimize_map call, recorded in run_log."""
