@@ -469,6 +469,61 @@ int nsb_mesh_clean(const double* vertices, int n_vertices, const int32_t* faces,
 int nsb_mesh_compact(const double* vertices, int n_vertices, const int32_t* faces, int n_faces, const void* workspace,
                      double* out_vertices, int32_t* out_faces, void* stream);
 
+/* ---- reconstruction metrics (calc_3d_metric, src/tools/eval_recon.py:91-117, and get_align_transformation, :45-59; nsb_recon.cu) --------
+ * Everything is float64; vertices and points are device f64 [n][3], faces device int32 [F][3] with indices the caller has checked. */
+
+/* trimesh.sample.sample_surface (trimesh 3.10.7) with the caller's uniforms f64 [count][3] = (u0, u1, u2) in place of its two np.random
+ * draws: area_f = sqrt(c.x^2 + c.y^2 + c.z^2) / 2, c = (v1 - v0) x (v2 - v0) (numpy's order); cum = inclusive scan of the areas (the
+ * excl_scan of nsb_scan.cuh: a fixed order, not numpy's sequential cumsum, so a pick within rounding of a boundary may choose the
+ * neighbouring face); face = searchsorted(cum, u0 * cum[F-1], 'left'); (a, b) = (u1, u2), (|a - 1|, |b - 1|) if a + b > 1;
+ * point = (a (v1 - v0) + b (v2 - v0)) + v0.  -> points f64 [count][3], face_index int64 [count].  n_faces >= 1. */
+size_t nsb_sample_surface_workspace(int n_faces);
+int nsb_sample_surface(const double* vertices, const int32_t* faces, int n_faces, const double* uniforms, long long count,
+                       void* workspace, size_t workspace_bytes, double* points, long long* face_index, void* stream);
+
+/* Exact nearest neighbours (the role of scipy's cKDTree in eval_recon.py) on a uniform grid of cubic cells over the targets' bounding
+ * box [lo, hi] (extents e = hi - lo, E = max e):
+ *   cell = cbrt(prod_a max(e_a, E/64) / N), then grown by 2^(1/8) until prod_a (floor(e_a / cell) + 1) <= 2 N -- so at most 2 N cells
+ *   whatever the spread (one far outlier makes the cells large, not many); E = 0: cell = 1, one cell.
+ *   dims_a = floor(e_a / cell) + 1, origin = lo; a point's cell along a is floor((x_a - lo_a) / cell) clamped to [0, dims_a - 1].
+ *   slack = 16 DBL_EPSILON (max |lo|, |hi| + E + cell) widens every cell box in the search's distance bounds, so that a point rounded
+ *   into a neighbouring cell is still found.
+ * Three steps: nsb_nn_bounds (box f64 [6] = lo, hi on the device) -> nsb_nn_plan (host: the rule above, fills origin, cell, slack,
+ * dims, n_cells, n_points) -> the caller allocates cell_start u64 [n_cells + 1], points f64 [N][3] and index int32 [N] -> nsb_nn_build
+ * (counting sort: counts, excl_scan, scatter; targets in cell order, index = their input position).  The order inside a cell depends on
+ * the scatter's atomics; no result does.
+ * nsb_nn_query: for each query (finite) the target with the least d2 = dx^2 + dy^2 + dz^2 (float64, no FMA), equal d2 -> the smaller
+ * index.  The search visits shells of cells around the query's clamped cell, skips cells whose box is farther than the best so far,
+ * and stops when no unvisited cell can hold a point at d2 <= best: exact also for queries outside the box.  radius >= 0 (finite): only
+ * targets with d2 < radius^2 count (scipy's distance_upper_bound rule), none -> index -1, dist2 = +inf; radius < 0 or infinite: no
+ * limit. */
+typedef struct {
+  double origin[3];
+  double cell;
+  double slack;
+  int32_t dims[3];
+  long long n_cells;
+  int32_t n_points;
+  unsigned long long* cell_start;   /* device [n_cells + 1]: targets of cell c are slots cell_start[c] .. cell_start[c + 1] - 1 */
+  double* points;                   /* device [n_points][3]: the targets in cell order */
+  int32_t* index;                   /* device [n_points]: input position of each slot */
+} nsb_nn_grid;
+size_t nsb_nn_bounds_workspace(int n_points);
+int nsb_nn_bounds(const double* points, int n_points, void* workspace, size_t workspace_bytes, double* box, void* stream);
+int nsb_nn_plan(const double box[6], int n_points, nsb_nn_grid* grid);
+size_t nsb_nn_build_workspace(long long n_cells);
+int nsb_nn_build(const double* targets, const nsb_nn_grid* grid, void* workspace, size_t workspace_bytes, void* stream);
+int nsb_nn_query(const nsb_nn_grid* grid, const double* queries, int n_queries, double radius, double* dist2, int32_t* index, void* stream);
+
+/* One correspondence pass of open3d 0.13's registration_icp with TransformationEstimationPointToPoint (GetRegistrationResultAndCorrespondences):
+ * every source point p = T[:3,:3] s + T[:3,3] (transform f64 [16], row-major 4x4, host; applied on the fly) is paired with its
+ * nsb_nn_query neighbour q within max_distance (d2 < max_distance^2).  sums f64 [17] (device) = [pairs, sum d2, sum p (3), sum q (3),
+ * sum p_i q_j (9, row i)].  Per-block partials (a fixed number of blocks for n_source), then one block sums them in block order: no
+ * float atomics, so two calls on the same input return the same bits. */
+size_t nsb_icp_workspace(int n_source);
+int nsb_icp_sums(const nsb_nn_grid* grid, const double* source, int n_source, const double transform[16], double max_distance,
+                 void* workspace, size_t workspace_bytes, double* sums, void* stream);
+
 /* Pose-gradient reduction: rays_d = sum_j dirs_j * R[:,j], rays_o = t (get_rays_from_uv, src/common.py:74-89) =>
  * d c2w[i][j] = sum_r d_rays_d[r][i] * dirs[r][j] (j<3), d c2w[i][3] = sum_r d_rays_o[r][i].  dirs: [N,3] camera-frame
  * directions.  d_c2w: float64 [3][4], OVERWRITTEN.  The quaternion chain (quad2rotation, src/common.py:137-160) stays in

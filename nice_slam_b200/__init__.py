@@ -6,6 +6,8 @@ Public surface:
     FusedMapper     one Mapper.optimize_map call on the fused path (mapping.py)
     FusedSLAM       a whole RGB-D sequence on the fused path, NICE_SLAM.run under strict sync (slam.py); ate_rmse
     FusedMesher     Mesher.get_mesh of a fused run's grids, decoders and keyframes on the GPU (mesh.py)
+    recon           eval_recon.py's 3D reconstruction metric on the GPU: nice_slam_b200.recon.eval_recon, or
+                    python -m nice_slam_b200.recon --rec_mesh A --gt_mesh B -3d (not imported here, so that -m runs it cleanly)
     to_channels_last, lib (ctypes handle of libnsb.so)
 """
 from ._lib import lib, LIB_PATH                       # noqa: F401

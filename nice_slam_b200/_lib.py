@@ -75,6 +75,11 @@ class MeshLattice(C.Structure):
                 ("planes", C.c_void_p), ("n_planes", C.c_int32)]
 
 
+class NNGrid(C.Structure):
+    _fields_ = [("origin", C.c_double * 3), ("cell", C.c_double), ("slack", C.c_double), ("dims", C.c_int32 * 3), ("n_cells", C.c_longlong),
+                ("n_points", C.c_int32), ("cell_start", C.c_void_p), ("points", C.c_void_p), ("index", C.c_void_p)]
+
+
 class Peers(C.Structure):
     _fields_ = [("rank", C.c_int), ("world", C.c_int), ("buffer", C.c_void_p * 8), ("counters", C.c_void_p), ("max_rays", C.c_int)]
 
@@ -153,6 +158,16 @@ SYMBOLS = {
     "nsb_mesh_clean_workspace": (C.c_size_t, [C.c_int, C.c_int]),
     "nsb_mesh_clean": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, C.c_size_t, _P, _P]),
     "nsb_mesh_compact": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
+    "nsb_sample_surface_workspace": (C.c_size_t, [C.c_int]),
+    "nsb_sample_surface": (C.c_int, [_P, _P, C.c_int, _P, C.c_longlong, _P, C.c_size_t, _P, _P, _P]),
+    "nsb_nn_bounds_workspace": (C.c_size_t, [C.c_int]),
+    "nsb_nn_bounds": (C.c_int, [_P, C.c_int, _P, C.c_size_t, _P, _P]),
+    "nsb_nn_plan": (C.c_int, [C.POINTER(C.c_double), C.c_int, C.POINTER(NNGrid)]),
+    "nsb_nn_build_workspace": (C.c_size_t, [C.c_longlong]),
+    "nsb_nn_build": (C.c_int, [_P, C.POINTER(NNGrid), _P, C.c_size_t, _P]),
+    "nsb_nn_query": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.c_double, _P, _P, _P]),
+    "nsb_icp_workspace": (C.c_size_t, [C.c_int]),
+    "nsb_icp_sums": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.POINTER(C.c_double), C.c_double, _P, C.c_size_t, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),
     "nsb_batch_max_depth_peers": (C.c_int, [_P, C.c_int, _P, C.POINTER(Peers), _P]),
     "nsb_tracking_seeds_peers": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(Peers), _P, _P, _P, _P, C.c_size_t, _P]),

@@ -5,6 +5,7 @@
 #include <cstring>
 #include "nsb_common.cuh"
 #include "nsb_mc_table.h"
+#include "nsb_scan.cuh"
 
 namespace nsb {
 namespace {
@@ -25,53 +26,6 @@ int upload_table() {
   return NSB_OK;
 }
 unsigned blocks_for(long long n) { return (unsigned)((n + kThreads - 1) / kThreads); }
-
-// ---- exclusive scan of u64 counts, in place: x[i] <- sum_{j<i} x[j] (three kernels per level, block sums scanned recursively) ----------
-constexpr int kScanItems = 4;                       // per thread
-constexpr long long kScanBlock = (long long)kThreads * kScanItems;
-__device__ __forceinline__ unsigned long long block_excl_scan(unsigned long long v, unsigned long long* total) {
-  __shared__ unsigned long long s_w[kThreads / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned long long inc = v;
-  for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-  if (lane == 31) s_w[warp] = inc;
-  __syncthreads();
-  unsigned long long base = 0, all = 0;
-  for (int w = 0; w < kThreads / 32; w++) { if (w < warp) base += s_w[w]; all += s_w[w]; }
-  __syncthreads();
-  *total = all;
-  return base + inc - v;
-}
-__global__ void scan_blocks_kernel(unsigned long long* x, long long n, unsigned long long* sums) {
-  const long long b0 = (long long)blockIdx.x * kScanBlock + (long long)threadIdx.x * kScanItems;
-  unsigned long long v[kScanItems], s = 0;
-#pragma unroll
-  for (int i = 0; i < kScanItems; i++) { v[i] = b0 + i < n ? x[b0 + i] : 0ull; s += v[i]; }
-  unsigned long long total;
-  unsigned long long run = block_excl_scan(s, &total);
-#pragma unroll
-  for (int i = 0; i < kScanItems; i++) { if (b0 + i < n) x[b0 + i] = run; run += v[i]; }
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-__global__ void scan_add_kernel(unsigned long long* x, long long n, const unsigned long long* sums) {
-  const long long i = (long long)blockIdx.x * kScanBlock + threadIdx.x;
-  for (int k = 0; k < kScanItems; k++) { const long long j = i + (long long)k * kThreads; if (j < n) x[j] += sums[blockIdx.x]; }
-}
-size_t scan_ws_elems(long long n) {
-  size_t t = 0;
-  for (long long m = n; m > 1; m = (m + kScanBlock - 1) / kScanBlock) t += (size_t)((m + kScanBlock - 1) / kScanBlock);
-  return t + 1;
-}
-int excl_scan(unsigned long long* x, long long n, unsigned long long* ws, cudaStream_t st) {
-  if (n <= 0) return NSB_OK;
-  const long long nb = (n + kScanBlock - 1) / kScanBlock;
-  scan_blocks_kernel<<<(unsigned)nb, kThreads, 0, st>>>(x, n, ws);
-  if (nb > 1) {
-    int rc = excl_scan(ws, nb, ws + nb, st); if (rc) return rc;
-    scan_add_kernel<<<(unsigned)nb, kThreads, 0, st>>>(x, n, ws);
-  }
-  return check_cuda(cudaGetLastError(), "mesh scan");
-}
 
 // ---- marching cubes ----------------------------------------------------------------------------------------------------------------
 struct Lat { int nx, ny, nz; long long N; };
