@@ -1269,8 +1269,8 @@ static size_t tile_wg_smem_bytes() { return tl::kWgBytes + ((tile_smem_bytes(tru
 
 // ---- which kernel family serves a call --------------------------------------------------------------------------------------------
 // mlp_backend 3: the tile kernels; 2: the round-1 ray-group kernels; 1: FP32-FMA; 0 (auto): the tile kernels, except batches of up to
-// small_rays rays (default 0 = never: the tile kernels are level with the ray-group ones at 200 rays -- 0.1105 ms per tracking iteration
-// either way, r02j / r02l -- and ahead everywhere else).  The tile kernels take tl::kMinSamples <= S <= NSB_MAX_SAMPLES, the ray-group
+// small_rays rays (default 0 = never; H100 tracking iteration, README "decoder back-ends": the ray-group kernels lead by 3-7 us at 16 and
+// 64 rays, the tile kernels by ~20 % from 200 rays on).  The tile kernels take tl::kMinSamples <= S <= NSB_MAX_SAMPLES, the ray-group
 // kernels S <= kMaxPtsTc; other calls fall to FP32-FMA.  Points mode follows mlp_backend alone.  Forward and backward of an iteration see
 // the same (S, n_rays) and so pick the same family (the saved ReLU bits are laid out per family).
 static int g_small_rays = 0;
