@@ -458,6 +458,20 @@ int nsb_mesh_depth_limits(const float* depth, int M, long long hw, float* depth_
 int nsb_mesh_seen(const double* vertices, int n_vertices, const float* w2c, int M, const float* depth_limit, double fx, double fy,
                   double cx, double cy, int H, int W, uint8_t* seen, void* stream);
 
+/* ---- ground-truth culling (src/tools/cull_mesh.py:47-75; nsb_mesh.cu) ---------------------------------------------------------------
+ * nsb_cull_seen: seen u8 [V] = 1 iff some pose of w2c f32 [P][16] (row-major; rows 0-2 are read) sees the vertex, with the projection of
+ * nsb_mesh_seen but z = uv.z + 1e-5f and no depth limit: 0 < uv.x/z < W && 0 < uv.y/z < H && z < 0 (cull_mesh.py's 0 <= -z: at z = 0
+ * the divisions fail the u test).  A pose with a NaN entry sees nothing.  P = 0: nothing is seen.  fx .. cy are rounded to float32.
+ * nsb_cull_faces: keep face f iff any of its vertices is seen (faces device int32 [F][3], indices the caller has checked in [0, V));
+ * totals[0] = kept faces (device int64).  nsb_cull_faces_emit with the same workspace: kept int32 [totals[0]] = the kept face indices in
+ * ascending order.  Every vertex stays (trimesh's update_faces keeps them all). */
+int nsb_cull_seen(const double* vertices, int n_vertices, const float* w2c, int P, double fx, double fy, double cx, double cy, int H, int W,
+                  uint8_t* seen, void* stream);
+size_t nsb_cull_faces_workspace(int n_faces);
+int nsb_cull_faces(const int32_t* faces, int n_faces, const uint8_t* seen, void* workspace, size_t workspace_bytes, long long* totals,
+                   void* stream);
+int nsb_cull_faces_emit(int n_faces, const void* workspace, int32_t* kept, void* stream);
+
 /* Culling, shared-edge components and compaction (Mesher.py:469-511): a face is dropped iff its three vertices are unseen; faces sharing
  * an edge (an unordered vertex pair) are connected; component areas are float64 sums of the face areas (atomic: their order, and so the
  * last bit, may vary between calls); components with area > threshold are kept, or with largest != 0 only the largest.  nsb_mesh_clean:

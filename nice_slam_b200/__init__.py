@@ -8,6 +8,8 @@ Public surface:
     FusedMesher     Mesher.get_mesh of a fused run's grids, decoders and keyframes on the GPU (mesh.py)
     recon           eval_recon.py's 3D reconstruction metric on the GPU: nice_slam_b200.recon.eval_recon, or
                     python -m nice_slam_b200.recon --rec_mesh A --gt_mesh B -3d (not imported here, so that -m runs it cleanly)
+    cull            cull_mesh.py's ground-truth culling on the GPU: nice_slam_b200.cull.cull_mesh, or
+                    python -m nice_slam_b200.cull --input_mesh A --traj traj.txt --output_mesh B (not imported here either)
     to_channels_last, lib (ctypes handle of libnsb.so)
 """
 from ._lib import lib, LIB_PATH                       # noqa: F401

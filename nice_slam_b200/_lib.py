@@ -158,6 +158,10 @@ SYMBOLS = {
     "nsb_mesh_clean_workspace": (C.c_size_t, [C.c_int, C.c_int]),
     "nsb_mesh_clean": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, C.c_size_t, _P, _P]),
     "nsb_mesh_compact": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
+    "nsb_cull_seen": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, _P, _P]),
+    "nsb_cull_faces_workspace": (C.c_size_t, [C.c_int]),
+    "nsb_cull_faces": (C.c_int, [_P, C.c_int, _P, _P, C.c_size_t, _P, _P]),
+    "nsb_cull_faces_emit": (C.c_int, [C.c_int, _P, _P, _P]),
     "nsb_sample_surface_workspace": (C.c_size_t, [C.c_int]),
     "nsb_sample_surface": (C.c_int, [_P, _P, C.c_int, _P, C.c_longlong, _P, C.c_size_t, _P, _P, _P]),
     "nsb_nn_bounds_workspace": (C.c_size_t, [C.c_int]),

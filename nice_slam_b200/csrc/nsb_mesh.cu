@@ -181,6 +181,22 @@ __global__ void depth_limits_kernel(const float* depth, long long hw, float* out
     out[blockIdx.x] = __fmul_rn(m, 1.1f);                                   // torch.max(depth) * 1.1 (Mesher.py:179)
   }
 }
+// The projection of point_masks (Mesher.py:131-150) and cull_mesh.py (:51-67) in float32: T = rows 0-2 of a row-major w2c (12 floats
+// used); cam = T [p, 1]; cam.x = -cam.x; uv = K cam; z = uv.z + eps; inside iff 0 < uv.x/z < W, 0 < uv.y/z < H, z < 0.  cull_mesh.py
+// tests 0 <= -z: at z = +-0 the divisions give inf or NaN, which fail the u test, so z < 0 decides the same.  cam_z = cam.z.
+__device__ __forceinline__ bool in_frustum(const float* T, const float p[3], float fx, float fy, float cx, float cy, float H, float W,
+                                           float eps, float& cam_z) {
+  float c[3];
+  for (int r = 0; r < 3; r++)                                               // w2c @ [p, 1]
+    c[r] = __fmaf_rn(T[4 * r + 3], 1.0f, __fmaf_rn(T[4 * r + 2], p[2], __fmaf_rn(T[4 * r + 1], p[1], __fmul_rn(T[4 * r], p[0]))));
+  c[0] = -c[0];                                                             // cam_cord[:, 0] *= -1
+  const float u0 = __fmaf_rn(cx, c[2], __fmul_rn(fx, c[0]));               // K @ cam (zero entries add nothing)
+  const float v0 = __fmaf_rn(cy, c[2], __fmul_rn(fy, c[1]));
+  const float z = __fadd_rn(c[2], eps);
+  const float u = __fdiv_rn(u0, z), vv = __fdiv_rn(v0, z);
+  cam_z = c[2];
+  return u < W && u > 0.0f && vv < H && vv > 0.0f && z < 0.0f;
+}
 __global__ void seen_kernel(const double* verts, int n, const float* w2c, int M, const float* lim, float fx, float fy, float cx, float cy,
                             float H, float W, uint8_t* seen) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -188,20 +204,44 @@ __global__ void seen_kernel(const double* verts, int n, const float* w2c, int M,
   const float p[3] = {(float)verts[3 * v], (float)verts[3 * v + 1], (float)verts[3 * v + 2]};
   uint8_t s = 0;
   for (int m = 0; m < M && !s; m++) {
-    const float* T = w2c + 16 * m;
-    float c[3];
-    for (int r = 0; r < 3; r++)                                             // w2c @ [p, 1] (Mesher.py:131-136)
-      c[r] = __fmaf_rn(T[4 * r + 3], 1.0f, __fmaf_rn(T[4 * r + 2], p[2], __fmaf_rn(T[4 * r + 1], p[1], __fmul_rn(T[4 * r], p[0]))));
-    c[0] = -c[0];                                                           // cam_cord[:, 0] *= -1
-    const float u0 = __fmaf_rn(cx, c[2], __fmul_rn(fx, c[0]));             // K @ cam (zero entries add nothing)
-    const float v0 = __fmaf_rn(cy, c[2], __fmul_rn(fy, c[1]));
-    const float z = __fadd_rn(c[2], 1e-8f);
-    const float u = __fdiv_rn(u0, z), vv = __fdiv_rn(v0, z);
-    bool ok = u < W && u > 0.0f && vv < H && vv > 0.0f && z < 0.0f;
-    if (lim != nullptr) ok = ok && (-c[2] < lim[m]);
+    float cz;
+    bool ok = in_frustum(w2c + 16 * m, p, fx, fy, cx, cy, H, W, 1e-8f, cz);
+    if (lim != nullptr) ok = ok && (-cz < lim[m]);
     s = ok;
   }
   seen[v] = s;
+}
+
+// ---- cull_mesh.py -------------------------------------------------------------------------------------------------------------------
+// One thread per vertex over P poses.  Rows 0-2 of the poses are staged in shared memory kCullPoses at a time; a thread stops at the
+// first pose that sees its vertex, the block at the first tile boundary where all its vertices are seen (threads past V count as seen).
+constexpr int kCullPoses = 256;
+__global__ void __launch_bounds__(kThreads) cull_seen_kernel(const double* verts, int n, const float* w2c, int P, float fx, float fy,
+                                                             float cx, float cy, float H, float W, uint8_t* seen) {
+  __shared__ float s_T[kCullPoses * 12];
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  float p[3] = {0.0f, 0.0f, 0.0f};
+  if (v < n) { p[0] = (float)verts[3 * v]; p[1] = (float)verts[3 * v + 1]; p[2] = (float)verts[3 * v + 2]; }
+  bool s = v >= n;
+  for (int base = 0; base < P; base += kCullPoses) {
+    if (__syncthreads_and(s)) break;                                        // also: every thread is done with the previous tile
+    const int np = P - base < kCullPoses ? P - base : kCullPoses;
+    for (int i = threadIdx.x; i < 12 * np; i += blockDim.x) s_T[i] = w2c[16ll * base + 16 * (i / 12) + i % 12];
+    __syncthreads();
+    for (int m = 0; m < np && !s; m++) { float cz; s = in_frustum(s_T + 12 * m, p, fx, fy, cx, cy, H, W, 1e-5f, cz); }
+  }
+  if (v < n) seen[v] = s;
+}
+// keep[f] = 1 iff a vertex of face f is seen (f < F); keep[F] = 0, so that the exclusive scan ends in the total
+__global__ void cull_flag_kernel(const int* faces, int F, const uint8_t* seen, unsigned long long* keep) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > F) return;
+  keep[f] = f < F && (seen[faces[3 * f]] || seen[faces[3 * f + 1]] || seen[faces[3 * f + 2]]);
+}
+__global__ void cull_totals_kernel(const unsigned long long* scanned, int F, long long* totals) { totals[0] = (long long)scanned[F]; }
+__global__ void cull_emit_kernel(const unsigned long long* scanned, int F, int* kept) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f < F && scanned[f + 1] != scanned[f]) kept[scanned[f]] = f;
 }
 
 // ---- culling, components, compaction ----------------------------------------------------------------------------------------------
@@ -424,6 +464,36 @@ extern "C" int nsb_mesh_seen(const double* vertices, int n, const float* w2c, in
   seen_kernel<<<blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(vertices, n, w2c, M, lim, (float)fx, (float)fy, (float)cx, (float)cy,
                                                                      (float)H, (float)W, seen);
   return check_cuda(cudaGetLastError(), "seen_kernel launch");
+}
+
+// cull_mesh.py:47-75: the seen mask over every pose, then the faces with a seen vertex
+extern "C" int nsb_cull_seen(const double* vertices, int n, const float* w2c, int P, double fx, double fy, double cx, double cy, int H, int W,
+                             uint8_t* seen, void* stream) {
+  if (n < 0 || P < 0 || (n > 0 && (!vertices || !seen || (P > 0 && !w2c)))) { set_error("nsb_cull_seen: NULL pointer or negative count"); return NSB_ERR_ARG; }
+  if (H < 1 || W < 1 || !isfinite(fx) || !isfinite(fy) || !isfinite(cx) || !isfinite(cy)) {
+    set_error("nsb_cull_seen: H and W must be >= 1 and the intrinsics finite (H %d, W %d)", H, W); return NSB_ERR_ARG; }
+  if (n == 0) return NSB_OK;
+  cull_seen_kernel<<<blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(vertices, n, w2c, P, (float)fx, (float)fy, (float)cx, (float)cy,
+                                                                         (float)H, (float)W, seen);
+  return check_cuda(cudaGetLastError(), "cull_seen_kernel launch");
+}
+extern "C" size_t nsb_cull_faces_workspace(int F) { return F < 0 ? 0 : align16(8ull * (F + 1)) + 8ull * scan_ws_elems((long long)F + 1); }
+extern "C" int nsb_cull_faces(const int32_t* faces, int F, const uint8_t* seen, void* ws, size_t ws_bytes, long long* totals, void* stream) {
+  if (F < 0 || !ws || !totals || (F > 0 && (!faces || !seen))) { set_error("nsb_cull_faces: NULL pointer or negative count"); return NSB_ERR_ARG; }
+  if (ws_bytes < nsb_cull_faces_workspace(F)) { set_error("nsb_cull_faces: workspace %zu < %zu bytes", ws_bytes, nsb_cull_faces_workspace(F)); return NSB_ERR_ARG; }
+  const cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* keep = static_cast<unsigned long long*>(ws);
+  cull_flag_kernel<<<blocks_for((long long)F + 1), kThreads, 0, st>>>(faces, F, seen, keep);
+  int rc = check_cuda(cudaGetLastError(), "cull_flag_kernel launch"); if (rc) return rc;
+  if ((rc = excl_scan(keep, (long long)F + 1, reinterpret_cast<unsigned long long*>(static_cast<char*>(ws) + align16(8ull * (F + 1))), st))) return rc;
+  cull_totals_kernel<<<1, 1, 0, st>>>(keep, F, totals);
+  return check_cuda(cudaGetLastError(), "cull_totals_kernel launch");
+}
+extern "C" int nsb_cull_faces_emit(int F, const void* ws, int32_t* kept, void* stream) {
+  if (F < 0 || !ws || (F > 0 && !kept)) { set_error("nsb_cull_faces_emit: NULL pointer or negative count"); return NSB_ERR_ARG; }
+  if (F == 0) return NSB_OK;
+  cull_emit_kernel<<<blocks_for(F), kThreads, 0, (cudaStream_t)stream>>>(static_cast<const unsigned long long*>(ws), F, kept);
+  return check_cuda(cudaGetLastError(), "cull_emit_kernel launch");
 }
 
 // culling + trimesh's split + the area filter + compaction (Mesher.py:469-511)

@@ -2,6 +2,7 @@
 (calc_3d_metric, :91-117, with get_align_transformation, :45-59), which needs trimesh and open3d on the host.
 
   read_ply           binary little-endian triangle meshes (mesh.write_ply's, trimesh's and open3d's), validated
+  read_ply_records   the same files as their header lines and raw records per element; write_ply_records writes them back
   sample_surface     trimesh.sample.sample_surface on the device (nsb_sample_surface), uniforms from a torch.Generator
   NearestNeighbours  exact nearest neighbours on a uniform grid (nsb_nn_*), the role of scipy's cKDTree in eval_recon.py
   icp_align          open3d 0.13's registration_icp, point to point (nsb_icp_sums per iteration, the 3x3 SVD on the host)
@@ -12,6 +13,7 @@ python -m nice_slam_b200.recon --rec_mesh A.ply --gt_mesh B.ply -3d   prints eva
 """
 import argparse
 import ctypes as C
+import os
 import sys
 
 import numpy as np
@@ -32,13 +34,17 @@ def _ply_type(name, what):
 
 
 def _parse_header(fh, path):
+    """-> (header lines as read, line ends included, up to and including end_header; [(name, count, [property words])])."""
     if fh.readline().strip() != b"ply":
         raise ValueError("read_ply: %s is not a PLY file" % path)
+    fh.seek(0)
+    lines = [fh.readline()]
     elements, fmt = [], None
     while True:
         line = fh.readline()
         if not line:
             raise ValueError("read_ply: %s ends before end_header" % path)
+        lines.append(line)
         w = line.decode("ascii", "replace").split()
         if not w or w[0] in ("comment", "obj_info"):
             continue
@@ -54,7 +60,7 @@ def _parse_header(fh, path):
             raise ValueError("read_ply: %s: malformed header line %r" % (path, line.strip()))
     if fmt != "binary_little_endian":
         raise ValueError("read_ply: %s has format %r; only binary_little_endian is supported (not ascii or binary_big_endian)" % (path, fmt))
-    return elements
+    return lines, elements
 
 
 def _scalar_dtype(name, count, props, path):
@@ -66,59 +72,76 @@ def _scalar_dtype(name, count, props, path):
     return np.dtype(fields)
 
 
-def read_ply(path):
-    """-> (vertices f64 [V,3], faces int64 [F,3], colours uint8 [V,3] or None).  Binary little-endian only; vertex x / y / z as float
-    or double (other vertex properties are skipped by their sizes); faces as one list property with a uchar or int count and int or uint
-    indices, every face a triangle.  Anything else raises ValueError naming the element or property."""
+def _open_records(path):
+    """Parse the header -> (header lines, an iterator over (name, property words, records) in file order).  Each element is checked as
+    the iterator reaches it, so a reader that consumes it element by element raises in file order."""
     with open(path, "rb") as fh:
-        elements = _parse_header(fh, path)
+        header, elements = _parse_header(fh, path)
         data = fh.read()
-    off, verts, faces, colors = 0, None, None, None
 
-    def take(dtype, n, what):
-        nonlocal off
-        need = dtype.itemsize * n
-        if off + need > len(data):
-            raise ValueError("read_ply: %s: element %r is truncated (%d bytes, %d left)" % (path, what, need, len(data) - off))
-        a = np.frombuffer(data, dtype=dtype, count=n, offset=off)
-        off += need
-        return a
+    def records():
+        off = 0
+        for name, n, props in elements:
+            if n < 0:
+                raise ValueError("read_ply: %s: element %r has a negative count" % (path, name))
+            if name == "face":
+                lists = [p for p in props if p[0] == "list"]
+                if len(lists) != 1 or lists[0][-1] not in ("vertex_indices", "vertex_index"):
+                    raise ValueError("read_ply: %s: element 'face' needs one list property vertex_indices" % path)
+                fields = []
+                for p in props:
+                    if p[0] == "list":
+                        ct, it = p[1], p[2]
+                        if ct not in ("uchar", "uint8", "int", "int32", "uint", "uint32"):
+                            raise ValueError("read_ply: %s: face list count type %r (uchar or int expected)" % (path, ct))
+                        if it not in ("int", "int32", "uint", "uint32"):
+                            raise ValueError("read_ply: %s: face list index type %r (int or uint expected)" % (path, it))
+                        fields += [("__n", _ply_type(ct, "face count")), ("__i", _ply_type(it, "face index"), (3,))]
+                    else:
+                        fields.append((p[1], _ply_type(p[0], "property face.%s" % p[1])))
+                dt = np.dtype(fields)
+            else:
+                dt = _scalar_dtype(name, n, props, path)
+            need = dt.itemsize * n
+            if off + need > len(data):
+                raise ValueError("read_ply: %s: element %r is truncated (%d bytes, %d left)" % (path, name, need, len(data) - off))
+            rec = np.frombuffer(data, dtype=dt, count=n, offset=off)
+            off += need
+            if name == "face":
+                bad = np.nonzero(rec["__n"] != 3)[0]
+                if len(bad):
+                    raise ValueError("read_ply: %s: face %d has %d vertices; only triangles are supported" % (path, bad[0], rec["__n"][bad[0]]))
+            yield name, props, rec
 
-    for name, n, props in elements:
-        if n < 0:
-            raise ValueError("read_ply: %s: element %r has a negative count" % (path, name))
+    return header, records()
+
+
+def read_ply_records(path):
+    """-> (header, elements): header = the header's lines as read (bytes, line ends included, "ply" to "end_header"); elements = [(name,
+    property words, records)] in file order, records a read-only numpy structured array over the file's bytes (the face element's list
+    property is the fields __n (count) and __i (three indices)).  The formats and checks of read_ply's file layer: binary little-endian,
+    scalar properties, one triangle list property on 'face'; anything else raises ValueError as read_ply does.  write_ply_records writes
+    such a pair back."""
+    header, it = _open_records(path)
+    return header, list(it)
+
+
+def _mesh_of(path, elements):
+    """read_ply's arrays of the (name, props, records) of a file, checked in file order."""
+    verts, faces, colors = None, None, None
+    for name, props, rec in elements:
         if name == "face":
-            lists = [p for p in props if p[0] == "list"]
-            if len(lists) != 1 or lists[0][-1] not in ("vertex_indices", "vertex_index"):
-                raise ValueError("read_ply: %s: element 'face' needs one list property vertex_indices" % path)
-            fields = []
-            for p in props:
-                if p[0] == "list":
-                    ct, it = p[1], p[2]
-                    if ct not in ("uchar", "uint8", "int", "int32", "uint", "uint32"):
-                        raise ValueError("read_ply: %s: face list count type %r (uchar or int expected)" % (path, ct))
-                    if it not in ("int", "int32", "uint", "uint32"):
-                        raise ValueError("read_ply: %s: face list index type %r (int or uint expected)" % (path, it))
-                    fields += [("__n", _ply_type(ct, "face count")), ("__i", _ply_type(it, "face index"), (3,))]
-                else:
-                    fields.append((p[1], _ply_type(p[0], "property face.%s" % p[1])))
-            rec = take(np.dtype(fields), n, "face")
-            bad = np.nonzero(rec["__n"] != 3)[0]
-            if len(bad):
-                raise ValueError("read_ply: %s: face %d has %d vertices; only triangles are supported" % (path, bad[0], rec["__n"][bad[0]]))
             faces = rec["__i"].astype(np.int64)
-        else:
-            dt = _scalar_dtype(name, n, props, path)
-            rec = take(dt, n, name)
-            if name == "vertex":
-                for a in "xyz":
-                    if a not in dt.names:
-                        raise ValueError("read_ply: %s: element 'vertex' has no property %r" % (path, a))
-                    if dt[a] not in (np.dtype("<f4"), np.dtype("<f8")):
-                        raise ValueError("read_ply: %s: vertex property %r must be float or double" % (path, a))
-                verts = np.stack([rec[a].astype(np.float64) for a in "xyz"], 1)
-                if all(c in dt.names for c in ("red", "green", "blue")):
-                    colors = np.stack([rec[c] for c in ("red", "green", "blue")], 1).astype(np.uint8)
+        elif name == "vertex":
+            dt = rec.dtype
+            for a in "xyz":
+                if a not in dt.names:
+                    raise ValueError("read_ply: %s: element 'vertex' has no property %r" % (path, a))
+                if dt[a] not in (np.dtype("<f4"), np.dtype("<f8")):
+                    raise ValueError("read_ply: %s: vertex property %r must be float or double" % (path, a))
+            verts = np.stack([rec[a].astype(np.float64) for a in "xyz"], 1)
+            if all(c in dt.names for c in ("red", "green", "blue")):
+                colors = np.stack([rec[c] for c in ("red", "green", "blue")], 1).astype(np.uint8)
     if verts is None:
         raise ValueError("read_ply: %s has no element 'vertex'" % path)
     if faces is None:
@@ -128,6 +151,34 @@ def read_ply(path):
     if len(faces) and (faces.min() < 0 or faces.max() >= len(verts)):
         raise ValueError("read_ply: %s: face indices outside [0, %d)" % (path, len(verts)))
     return verts, faces, colors
+
+
+def read_ply(path):
+    """-> (vertices f64 [V,3], faces int64 [F,3], colours uint8 [V,3] or None).  Binary little-endian only; vertex x / y / z as float
+    or double (other vertex properties are skipped by their sizes); faces as one list property with a uchar or int count and int or uint
+    indices, every face a triangle.  Anything else raises ValueError naming the element or property."""
+    return _mesh_of(path, _open_records(path)[1])
+
+
+def write_ply_records(path, header, elements):
+    """Write read_ply_records' (header, elements), with any element's records replaced (e.g. a subset of the faces): the header's lines
+    unchanged except each 'element <name> <count>' line, whose count becomes the number of records given; then each element's records
+    as their bytes, in order.  Records taken from the file (or indexed subsets of them) come out byte for byte."""
+    counts = iter([len(rec) for _, _, rec in elements])
+    out = []
+    for line in header:
+        w = line.split()
+        if len(w) == 3 and w[0] == b"element":
+            end = line[len(line.rstrip(b"\r\n")):]
+            line = b"element %s %d" % (w[1], next(counts)) + end
+        out.append(line)
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    with open(path, "wb") as fh:
+        fh.write(b"".join(out))
+        for _, _, rec in elements:
+            fh.write(np.ascontiguousarray(rec).tobytes())
 
 
 # ---------------------------------------------------------------------------------------------- device steps
