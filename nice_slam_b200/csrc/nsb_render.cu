@@ -164,6 +164,7 @@ struct KParams {
   int* ray_cnt;                 // [N] completion counters of the rays, zero between launches (the completing CTA resets them)
   float4* tile_parts;           // forward: [split][N*S] per-item decoder outputs (split == 1: aliases fo.raw)
   int tile_rays;                // backward: rays one tile can touch (stride of ray_parts per item)
+  int kind_major;               // block order (tl::item_of_block): 1 = decoder-major (item_order), 0 = tile-major
   FusedSeeds fs;                // forward: loss seeds computed by the last CTA to finish (kind 0 = not fused)
   PeerTail tail;                // backward: sum of [loss | d c2w] over ranks by the last CTA (px.world <= 1: none)
   int acts_mask;                // levels whose layer outputs fo.acts / bw.acts hold, one [N*S][5][32] block each in level order (acts_slot)
@@ -1128,7 +1129,7 @@ static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.n_dec = stage_decoders(in->stage, K.dec);
   for (int i = 0; i < 3; i++) K.dec_pos[i] = i;
   K.accumulate_rays = 0;
-  K.split = 1; K.group_done = nullptr; K.fwd_parts = nullptr; K.ray_parts = nullptr; K.ray_cnt = nullptr; K.tile_parts = nullptr; K.tile_rays = 0;
+  K.split = 1; K.group_done = nullptr; K.fwd_parts = nullptr; K.ray_parts = nullptr; K.ray_cnt = nullptr; K.tile_parts = nullptr; K.tile_rays = 0; K.kind_major = 0;
   memset(&K.fs, 0, sizeof(K.fs)); memset(&K.tail, 0, sizeof(K.tail));
   K.wbytes = weight_bytes(K.dec, K.n_dec);
   K.points = nullptr; K.points_raw = nullptr; K.n_points = 0;
@@ -1200,8 +1201,17 @@ static size_t tile_scratch_bytes(int N, int S, int split, bool bwd) {
   return bwd ? (size_t)tile_count(NS) * split * tile_rays(S) * 6 * sizeof(double) : (split > 1 ? (size_t)split * NS * sizeof(float4) : 0);
 }
 static size_t tile_ws_need(int N, int S, int split, bool bwd) { return 16 + align16((size_t)N * sizeof(int)) + align16(tile_scratch_bytes(N, S, split, bwd)); }
-// The tile launch K in the caller's split workspace: items per tile (split), ray-completion counters, per-item scratch
-static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd) {
+// Block order of a launch of `tiles` x `split` items at ctas_per_sm resident CTAs per SM (tl::item_of_block).  When the whole launch is
+// resident at once, the block scheduler gives blocks 0 .. sms-1 one SM each; where the later blocks go does not follow that order
+// (tools/item_timing.py, H100, 225 blocks: block sms + j shares block j's SM 16 % of the time).  Such a launch takes its items decoder-major,
+// the fine decoder's first: its tiles <= sms fine items are then all in the first round, and no SM runs two of them (tile-major: the 200-ray
+// launches' last SM ran two fine items in 59 of 60 launches).  A launch of several rounds keeps tile-major order, which mixes the kinds in
+// every round (decoder-major: the 996-ray mapping backward, 748 items, ran 9 % slower).  Kernels of one CTA per SM share no SM: tile-major.
+static int item_order(long long tiles, int split, int ctas_per_sm) {
+  return ctas_per_sm > 1 && split > 1 && tiles * split <= (long long)ctas_per_sm * sm_count();
+}
+// The tile launch K in the caller's split workspace: items per tile (split), their block order, ray-completion counters, per-item scratch
+static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd, int ctas_per_sm) {
   const int N = K.in.n_rays, S = K.S, n_dec = K.n_dec;
   bytes &= ~size_t(15);
   int split = ((long long)N * S <= kSplitMaxPts && n_dec > 1) ? n_dec : 1;
@@ -1218,6 +1228,7 @@ static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd) {
   if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15) || bytes < tile_ws_need(N, S, split, bwd)) {
     set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", N, S); return NSB_ERR_ARG; }
   K.split = split;
+  K.kind_major = item_order(tile_count((long long)N * S), split, ctas_per_sm);
   K.ray_cnt = reinterpret_cast<int*>(static_cast<char*>(ws) + bytes - align16((size_t)N * sizeof(int)));
   if (bwd) { K.ray_parts = static_cast<double*>(ws); K.tile_rays = tile_rays(S); }
   else K.tile_parts = split > 1 ? static_cast<float4*>(ws) : reinterpret_cast<float4*>(K.fo.raw);
@@ -1409,7 +1420,7 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
     set_error("in-kernel exchanges of a sharded forward need a tensor-core back-end and <= %d rays per rank", NSB_INLINE_MAX_RAYS); return NSB_ERR_UNSUPPORTED; }
   if (fam == Family::Tile) {
     if (!out->z_vals || !out->raw) { set_error("the tensor-core forward needs z_vals and raw outputs"); return NSB_ERR_ARG; }
-    if ((rc = plan_tile_ws(K, out->split_workspace, out->split_workspace_bytes, false))) return rc;
+    if ((rc = plan_tile_ws(K, out->split_workspace, out->split_workspace_bytes, false, 2))) return rc;
     return launch_tile_fwd(K, (long long)in->n_rays * K.S, (cudaStream_t)stream);
   }
   if (fam == Family::Group) return launch_group(K, false, out->split_workspace, out->split_workspace_bytes, (cudaStream_t)stream);
@@ -1550,7 +1561,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     const unsigned tiles = (unsigned)tile_count((long long)in->n_rays * P.S);
     if (kind[i] == GroupIg) rc = launch_group(P, true, bw->split_workspace, bw->split_workspace_bytes, st);
     else if (kind[i] == Fma) rc = launch_fma(P, true, st);
-    else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true))) return rc;
+    else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true, kind[i] == WgTile ? 1 : 2))) return rc;
     else if (kind[i] == WgTile && P.dec[0] == NSB_COARSE) {         // (stage coarse: the coarse decoder alone)
       render_bwd_wg_coarse_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
       rc = check_cuda(cudaGetLastError(), "render_bwd_wg_coarse_tile_kernel launch");
@@ -1607,6 +1618,22 @@ extern "C" int nsb_debug_occupancy(int* fwd, int* bwd) {
 extern "C" int nsb_debug_phases(long long* out64, int reset) {
   cudaError_t e = cudaMemcpyFromSymbol(out64, nsb::tc::g_phase, sizeof(long long) * 64);
   if (e == cudaSuccess && reset) { long long z[64] = {0}; e = cudaMemcpyToSymbol(nsb::tc::g_phase, z, sizeof(z)); }
+  return e == cudaSuccess ? 0 : 1;
+}
+#endif
+
+#ifdef NSB_ITEM_TIMING
+// the item records of the last launch of each kind (tl::item_mark): n records of `launch` (0 forward, 1 backward, 2 weight-gradient backward)
+// from block 0 on; reset = 1 clears all of them afterwards
+extern "C" int nsb_debug_items(int launch, void* out, int n, int reset) {
+  if (launch < 0 || launch > 2 || n < 0 || n > nsb::tl::kItemRecords) return 1;
+  const size_t rec = sizeof(nsb::tl::ItemRecord), all = sizeof(nsb::tl::g_items);
+  cudaError_t e = cudaMemcpyFromSymbol(out, nsb::tl::g_items, rec * n, rec * nsb::tl::kItemRecords * launch);
+  if (e == cudaSuccess && reset) {
+    void* p = nullptr;
+    e = cudaGetSymbolAddress(&p, nsb::tl::g_items);
+    if (e == cudaSuccess) e = cudaMemset(p, 0, all);
+  }
   return e == cudaSuccess ? 0 : 1;
 }
 #endif

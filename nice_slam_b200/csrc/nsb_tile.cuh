@@ -1073,6 +1073,47 @@ __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restric
   }
 }
 
+// ---- block -> item -----------------------------------------------------------------------------------------------------------------
+// Block b of a launch of tiles x split items runs item (tile, my): decoder-major (P.kind_major, item_order in nsb_render.cu) b = my * tiles +
+// tile, so the decoders come in their evaluation order, the fine decoder -- the slowest item: two grids, eight fc_c units -- first;
+// tile-major b = tile * split + my.  split == 1: block = tile either way.  Results do not depend on the order: the forward composites from
+// the per-decoder parts in decoder order, the backward adds the ray parts in (tile, decoder) order.  kShared = false: kernels of one CTA per
+// SM, which share no SM and so run tile-major (item_order never picks decoder-major for them).
+struct Item { int tile, my; };
+template <bool kShared = true>
+__device__ __forceinline__ Item item_of_block(const KParams& P, int b) {
+  if constexpr (!kShared) {
+    const int tile = b / P.split;
+    return {tile, b - tile * P.split};
+  }
+  const int d = P.kind_major ? (int)gridDim.x / P.split : P.split;
+  const int q = b / d, r = b - q * d;
+  return P.kind_major ? Item{r, q} : Item{q, r};
+}
+
+// Optional item timing (make ../libnsb_items.so, tools/item_timing.py): thread 0 of every tile CTA records its SM, its item and the global
+// timer at start, at the end of its decoder chain and at exit, per launch kind (0 forward, 1 backward, 2 weight-gradient backward); read
+// back with nsb_debug_items().  Compiled out of the product library.
+#ifdef NSB_ITEM_TIMING
+constexpr int kItemRecords = 16384;
+struct ItemRecord { int sm, tile, my, level; unsigned long long t[3]; };
+__device__ ItemRecord g_items[3][kItemRecords];
+__device__ __forceinline__ void item_mark(int launch, int k, const KParams& P, const Item& it) {
+  if (threadIdx.x != 0 || blockIdx.x >= kItemRecords) return;
+  ItemRecord& r = g_items[launch][blockIdx.x];
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
+  r.t[k] = t;
+  if (k == 0) {
+    int sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    r.sm = sm; r.tile = it.tile; r.my = it.my; r.level = P.split > 1 ? P.dec[it.my] : -1;
+  }
+}
+#define NSB_ITEM_MARK(launch, k, P, it) ::nsb::tl::item_mark(launch, k, P, it)
+#else
+#define NSB_ITEM_MARK(launch, k, P, it) do { } while (0)
+#endif
+
 // ---- tile <-> ray bookkeeping ------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int tiles_of_ray(int ray, int S) {
   const long long p0 = (long long)ray * S;
@@ -1146,7 +1187,9 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P, const Mes
 
   const bool points = kMesh || P.points != nullptr;
   const int nsplit = P.split;
-  const int tile = blockIdx.x / nsplit, my = blockIdx.x - tile * nsplit;
+  const Item item = item_of_block(P, blockIdx.x);
+  const int tile = item.tile, my = item.my;
+  NSB_ITEM_MARK(0, 0, P, item);
   const int q0 = nsplit > 1 ? my : 0, q1 = nsplit > 1 ? my + 1 : P.n_dec;
   const long long NP = points ? (long long)P.n_points : (long long)P.in.n_rays * P.S;
   const long long gp0 = (long long)tile * TM;
@@ -1235,6 +1278,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P, const Mes
   // set up under the ray compositing / loss-seed tail (triggering at kernel start made the early backward CTAs compete with the chain: slower)
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   NSB_PH(14);
+  NSB_ITEM_MARK(0, 1, P, item);
 
   if (points) {                                                   // Renderer.eval_points: raw with the out-of-bound override
     if (cg == 0 && row < npts) {
@@ -1249,6 +1293,7 @@ __device__ __forceinline__ void render_fwd_tile_body(const KParams& P, const Mes
   for (int k = warp; k < nd; k += kThreads / 32) composite_ray(P, s_done[k], lane, smem_raw + (size_t)warp * composite_scratch_bytes(S));
   NSB_PH(16);
   fused_seeds_tail(P, gridDim.x, smem_raw);                       // the last CTA of the grid to get here sees every ray composited
+  NSB_ITEM_MARK(0, 2, P, item);
 }
 __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_kernel(const __grid_constant__ KParams P) { render_fwd_tile_body<false>(P); }
 // forward with FP16 hi|lo operands (option fwd_f16; see mma_rows)
@@ -1282,7 +1327,9 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   wg.dpk = nullptr;
 
   const int nsplit = P.split;
-  const int tile = blockIdx.x / nsplit, my = blockIdx.x - tile * nsplit;
+  const Item item = item_of_block<WG == kWgNone>(P, blockIdx.x);
+  const int tile = item.tile, my = item.my;
+  NSB_ITEM_MARK(WG ? 2 : 1, 0, P, item);
   const int q0 = nsplit > 1 ? my : 0, q1 = nsplit > 1 ? my + 1 : P.n_dec;
   const int S = P.S;
   const long long NP = (long long)P.in.n_rays * S;
@@ -1375,6 +1422,7 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   }
   __syncthreads();
   if (threadIdx.x == 0) tc::acc_release(acc_slot);
+  NSB_ITEM_MARK(WG ? 2 : 1, 1, P, item);
 
   // per-ray sums of this item: d rays_o = sum_s dp, d rays_d = sum_s z_s dp (pts = o + d z, Renderer.py:172-174) -> global scratch
   const int RT = P.tile_rays;                                     // rays a tile can touch: stride of the per-item parts
@@ -1406,6 +1454,7 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
   }
   NSB_PH(32);
   if (fused_pose_grad(P, gridDim.x, reinterpret_cast<double*>(smem_raw))) pose_tail_peers(P);
+  NSB_ITEM_MARK(WG ? 2 : 1, 2, P, item);
 }
 __global__ void __launch_bounds__(tl::kThreads, 2) render_bwd_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<tl::kWgNone>(P); }
 __global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_kernel(const __grid_constant__ KParams P) { render_bwd_tile_body<tl::kWgXyz>(P); }
