@@ -472,6 +472,38 @@ int nsb_cull_faces(const int32_t* faces, int n_faces, const uint8_t* seen, void*
                    void* stream);
 int nsb_cull_faces_emit(int n_faces, const void* workspace, int32_t* kept, void* stream);
 
+/* ---- frame preparation (BaseDataset.__getitem__, src/utils/datasets.py:77-113; nsb_frame.cu) ---------------------------------------
+ * The raw decoded bytes of one frame -- colour BGR u8 [color_h][color_w][3] (cv2.imread), depth u16 [depth_h][depth_w] (IMREAD_UNCHANGED)
+ * -- to the prepared frame: colour f64 [H][W][3] RGB in [0, 1], depth f32 [H][W] (nsb_frame_output_size).  The reference's steps, in its
+ * order, each skipped when it does nothing:
+ *   1. undistort != 0: cv2.undistort(colour, K(fx, fy, cx, cy), dist[5] = k1 k2 p1 p2 k3), colour only.  Bit-identical to the map of
+ *      OpenCV's AVX2 dispatch of initUndistortRectifyMap (what cv2 runs on AVX2 and AVX-512 x86 hosts): stripes of max(1, 4096 / W) rows
+ *      with cy shifted by the stripe's first row, cv::invert's closed 3x3 form, the row walked in 8-column chunks, u = fma(fx, xd, cx);
+ *      the map rounded to 1/32 pixel, 15-bit bilinear weights, neighbours outside count as 0.  A build that dispatches another vector
+ *      width, or none, accumulates the row differently, and can round a map entry lying within an ulp of a 1/64-pixel tie the other way.
+ *   2. BGR -> RGB, / 255. in float64.
+ *   3. cv2.resize to the depth image's size when the sizes differ: INTER_LINEAR on float64 with float64 coefficients.  OpenCV's own
+ *      summation order is not reproduced (|difference| < 1e-13); at an exact 2x2 downscale OpenCV averages the 4 pixels (INTER_AREA),
+ *      which the bilinear weights of 1/2 equal up to rounding.
+ *   4. depth: float32(raw) / float32(png_depth_scale) * float32(scale), correctly rounded.
+ *   5. crop_h / crop_w != 0 (crop_size): colour F.interpolate bilinear align_corners=True in float64 (torch's CPU weights); depth
+ *      F.interpolate nearest with torch's float32 source index.
+ *   6. crop_edge pixels off every side.
+ * The workspace (nsb_frame_workspace bytes; 0 = none needed) holds the undistorted bytes and the full-size colour before crop_size. */
+typedef struct {
+  int color_h, color_w, depth_h, depth_w;
+  int undistort;
+  double fx, fy, cx, cy;               /* the configured camera, before crop_size / crop_edge (used by undistort only) */
+  double dist[5];
+  double png_depth_scale, scale;
+  int crop_h, crop_w;                  /* crop_size, or 0, 0 */
+  int crop_edge;
+} nsb_frame_params;
+void nsb_frame_output_size(const nsb_frame_params* f, int* H, int* W);
+size_t nsb_frame_workspace(const nsb_frame_params* f);
+int nsb_frame_prepare(const nsb_frame_params* f, const uint8_t* color_bgr, const uint16_t* depth_raw, void* workspace, size_t workspace_bytes,
+                      double* color_out, float* depth_out, void* stream);
+
 /* Culling, shared-edge components and compaction (Mesher.py:469-511): a face is dropped iff its three vertices are unseen; faces sharing
  * an edge (an unordered vertex pair) are connected; component areas are float64 sums of the face areas (atomic: their order, and so the
  * last bit, may vary between calls); components with area > threshold are kept, or with largest != 0 only the largest.  nsb_mesh_clean:

@@ -10,6 +10,9 @@ Public surface:
                     python -m nice_slam_b200.recon --rec_mesh A --gt_mesh B -3d (not imported here, so that -m runs it cleanly)
     cull            cull_mesh.py's ground-truth culling on the GPU: nice_slam_b200.cull.cull_mesh, or
                     python -m nice_slam_b200.cull --input_mesh A --traj traj.txt --output_mesh B (not imported here either)
+    build_scene     NICE_SLAM.__init__'s initial state (bound, grids, pretrained decoders, renderer) from a config (scene.py)
+    FrameReader     the reference's dataset readers, frames prepared on the GPU (datasets.py)
+    run             run.py's counterpart: python -m nice_slam_b200.run CONFIG (not imported here)
     to_channels_last, lib (ctypes handle of libnsb.so)
 """
 from ._lib import lib, LIB_PATH                       # noqa: F401
@@ -18,5 +21,7 @@ from .renderer import FusedRenderer, to_channels_last  # noqa: F401
 from .mapping import FusedMapper                       # noqa: F401
 from .mesh import FusedMesher                          # noqa: F401
 from .slam import FusedSLAM, ate_rmse                  # noqa: F401
+from .scene import build_scene                         # noqa: F401
+from .datasets import FrameReader                      # noqa: F401
 
-__all__ = ["FusedRenderer", "FusedMapper", "FusedSLAM", "FusedMesher", "ate_rmse", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH"]
+__all__ = ["FusedRenderer", "FusedMapper", "FusedSLAM", "FusedMesher", "ate_rmse", "build_scene", "FrameReader", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH"]

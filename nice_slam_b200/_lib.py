@@ -80,6 +80,12 @@ class NNGrid(C.Structure):
                 ("n_points", C.c_int32), ("cell_start", C.c_void_p), ("points", C.c_void_p), ("index", C.c_void_p)]
 
 
+class FrameParams(C.Structure):
+    _fields_ = [("color_h", C.c_int32), ("color_w", C.c_int32), ("depth_h", C.c_int32), ("depth_w", C.c_int32), ("undistort", C.c_int32),
+                ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double), ("dist", C.c_double * 5),
+                ("png_depth_scale", C.c_double), ("scale", C.c_double), ("crop_h", C.c_int32), ("crop_w", C.c_int32), ("crop_edge", C.c_int32)]
+
+
 class Peers(C.Structure):
     _fields_ = [("rank", C.c_int), ("world", C.c_int), ("buffer", C.c_void_p * 8), ("counters", C.c_void_p), ("max_rays", C.c_int)]
 
@@ -172,6 +178,9 @@ SYMBOLS = {
     "nsb_nn_query": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.c_double, _P, _P, _P]),
     "nsb_icp_workspace": (C.c_size_t, [C.c_int]),
     "nsb_icp_sums": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.POINTER(C.c_double), C.c_double, _P, C.c_size_t, _P, _P]),
+    "nsb_frame_output_size": (None, [C.POINTER(FrameParams), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "nsb_frame_workspace": (C.c_size_t, [C.POINTER(FrameParams)]),
+    "nsb_frame_prepare": (C.c_int, [C.POINTER(FrameParams), _P, _P, _P, C.c_size_t, _P, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),
     "nsb_batch_max_depth_peers": (C.c_int, [_P, C.c_int, _P, C.POINTER(Peers), _P]),
     "nsb_tracking_seeds_peers": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(Peers), _P, _P, _P, _P, C.c_size_t, _P]),

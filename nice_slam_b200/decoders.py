@@ -15,8 +15,10 @@ from ._lib import LEVELS
 HIDDEN, EMBED, C_DIM = 32, 93, 32
 
 
-def _xavier_linear(n_in, n_out, gain):
-    lin = nn.Linear(n_in, n_out)
+def _xavier_linear(n_in, n_out, gain, reference_draws=False):
+    """reference_draws: draw only xavier's uniforms, as DenseLayer (whose reset_parameters replaces nn.Linear's) does; otherwise
+    nn.Linear's own kaiming and bias draws come first."""
+    lin = nn.utils.skip_init(nn.Linear, n_in, n_out) if reference_draws else nn.Linear(n_in, n_out)
     nn.init.xavier_uniform_(lin.weight, gain=gain)      # DenseLayer.reset_parameters, decoder.py:77-82
     nn.init.zeros_(lin.bias)
     return lin
@@ -31,7 +33,7 @@ class _Embedder(nn.Module):
 class DecoderMLP(nn.Module):
     """Parameters of MLP (xyz=True; middle/fine/color) or MLP_no_xyz (xyz=False; coarse)."""
 
-    def __init__(self, name, xyz=True, c_dim=C_DIM, color=False):
+    def __init__(self, name, xyz=True, c_dim=C_DIM, color=False, reference_draws=False):
         super().__init__()
         self.name, self.xyz, self.c_dim, self.color = name, xyz, c_dim, color
         relu_gain = nn.init.calculate_gain("relu")
@@ -41,18 +43,22 @@ class DecoderMLP(nn.Module):
             ins = [EMBED, HIDDEN, HIDDEN, HIDDEN + EMBED, HIDDEN]
         else:
             ins = [HIDDEN, HIDDEN, HIDDEN, HIDDEN + c_dim, HIDDEN]
-        self.pts_linears = nn.ModuleList([_xavier_linear(i, HIDDEN, relu_gain) for i in ins])
-        self.output_linear = _xavier_linear(HIDDEN, 4 if color else 1, 1.0)
+        self.pts_linears = nn.ModuleList([_xavier_linear(i, HIDDEN, relu_gain, reference_draws) for i in ins])
+        self.output_linear = _xavier_linear(HIDDEN, 4 if color else 1, 1.0, reference_draws)
 
 
 class NICEDecoders(nn.Module):
-    def __init__(self, coarse=True):
+    def __init__(self, coarse=True, reference_draws=False):
+        """reference_draws: draw from torch's global generator exactly as config.get_model(cfg, nice=True) does (fc_c as nn.Linear, the
+        embedder's randn, then xavier only for pts_linears and output_linear; coarse, middle, fine, colour), so that under one seed the
+        parameters come out bit-identical to the reference's.  The default keeps this class's own draws."""
         super().__init__()
+        r = reference_draws
         if coarse:
-            self.coarse_decoder = DecoderMLP("coarse", xyz=False)
-        self.middle_decoder = DecoderMLP("middle")
-        self.fine_decoder = DecoderMLP("fine", c_dim=2 * C_DIM)
-        self.color_decoder = DecoderMLP("color", color=True)
+            self.coarse_decoder = DecoderMLP("coarse", xyz=False, reference_draws=r)
+        self.middle_decoder = DecoderMLP("middle", reference_draws=r)
+        self.fine_decoder = DecoderMLP("fine", c_dim=2 * C_DIM, reference_draws=r)
+        self.color_decoder = DecoderMLP("color", color=True, reference_draws=r)
 
     @classmethod
     def from_state(cls, state, device=None):
