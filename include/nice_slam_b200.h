@@ -570,6 +570,30 @@ size_t nsb_icp_workspace(int n_source);
 int nsb_icp_sums(const nsb_nn_grid* grid, const double* source, int n_source, const double transform[16], double max_distance,
                  void* workspace, size_t workspace_bytes, double* sums, void* stream);
 
+/* ---- 2D reconstruction metric (calc_2d_metric, src/tools/eval_recon.py:120-209; nsb_depth.cu) ---------------------------------------
+ * nsb_depth_render: z-depth of a triangle mesh (vertices device f64 [V][3], faces device int32 [F][3] with indices the caller has checked)
+ * under P cameras (c2w device f64 [P][16], row-major, OpenCV convention: x right, y down, z forward; rows 0-2 are read) -> depth f32
+ * [P][H][W].  The rule, in float64 camera space p_cam = R^T (p - t), for pixel (row i, column j) with ray d = ((j - cx)/fx, (i - cy)/fy, 1):
+ *   coverage: with the face's camera-space vertices a, b, c and D = N.a, N = (b - a) x (c - a): the ray is inside edge (u, v) iff
+ *     sgn(D) d.(u x v) > 0 (homogeneous rasterization: no near-plane clipping, vertices behind the camera allowed, both windings).  u x v
+ *     of an edge and v x u of its twin in a neighbouring face are exact negations, so both faces see the same value.  A ray with
+ *     d.(u x v) == 0 goes to the face on the positive side of the edge plane, its normal's sign chosen so that the first non-zero
+ *     component is positive: watertight across shared edges (and duplicated vertices at equal positions), and a ray through a vertex
+ *     goes to one face of its fan.  D == 0 (the face's plane holds the camera centre): no coverage.
+ *   depth: z = D / (N.d), the ray's intersection with the face's plane; a hit counts iff z_near <= z <= z_far.
+ *   pixel: the least z of its hits rounded to float32 (atomicMin on the bits: independent of the order faces arrive), 0 without a hit.
+ * 0 < z_near <= z_far < inf.  Workspace: nsb_depth_render_workspace(F, P) bytes (a queue of the faces whose pixel box is large).
+ * nsb_depth_l1: errors f64 [P] = mean over hw pixels of |a - b| in float64, a fixed summation order (repeats are bit-identical).
+ * nsb_views_see_any: any u8 [P] = 1 iff some point (device f64 [N][3]) is inside the frustum of pose p (w2c device f32 [P][16]) under
+ * the projection of nsb_cull_seen (z = uv.z + 1e-5f): check_proj, with w2c = float32(inv(float64 c2w with columns 1 and 2 negated)). */
+size_t nsb_depth_render_workspace(int n_faces, int P);
+int nsb_depth_render(const double* vertices, int n_vertices, const int32_t* faces, int n_faces, const double* c2w, int P, double fx,
+                     double fy, double cx, double cy, int H, int W, double z_near, double z_far, void* workspace, size_t workspace_bytes,
+                     float* depth, void* stream);
+int nsb_depth_l1(const float* depth_a, const float* depth_b, int P, long long hw, double* errors, void* stream);
+int nsb_views_see_any(const double* points, int n_points, const float* w2c, int P, double fx, double fy, double cx, double cy, int H, int W,
+                      uint8_t* any, void* stream);
+
 /* Pose-gradient reduction: rays_d = sum_j dirs_j * R[:,j], rays_o = t (get_rays_from_uv, src/common.py:74-89) =>
  * d c2w[i][j] = sum_r d_rays_d[r][i] * dirs[r][j] (j<3), d c2w[i][3] = sum_r d_rays_o[r][i].  dirs: [N,3] camera-frame
  * directions.  d_c2w: float64 [3][4], OVERWRITTEN.  The quaternion chain (quad2rotation, src/common.py:137-160) stays in

@@ -178,7 +178,12 @@ SYMBOLS = {
     "nsb_nn_query": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.c_double, _P, _P, _P]),
     "nsb_icp_workspace": (C.c_size_t, [C.c_int]),
     "nsb_icp_sums": (C.c_int, [C.POINTER(NNGrid), _P, C.c_int, C.POINTER(C.c_double), C.c_double, _P, C.c_size_t, _P, _P]),
-    "nsb_frame_output_size": (None, [C.POINTER(FrameParams), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "nsb_depth_render_workspace": (C.c_size_t, [C.c_int, C.c_int]),
+    "nsb_depth_render": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int,
+                                   C.c_double, C.c_double, _P, C.c_size_t, _P, _P]),
+    "nsb_depth_l1": (C.c_int, [_P, _P, C.c_int, C.c_longlong, _P, _P]),
+    "nsb_views_see_any": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, _P, _P]),
+    "nsb_frame_output_size":(None, [C.POINTER(FrameParams), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "nsb_frame_workspace": (C.c_size_t, [C.POINTER(FrameParams)]),
     "nsb_frame_prepare": (C.c_int, [C.POINTER(FrameParams), _P, _P, _P, C.c_size_t, _P, _P, _P]),
     "nsb_peer_buffer_bytes": (C.c_size_t, [C.c_int]),

@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstring>
 #include "nsb_common.cuh"
+#include "nsb_geom.cuh"
 #include "nsb_mc_table.h"
 #include "nsb_scan.cuh"
 
@@ -181,22 +182,7 @@ __global__ void depth_limits_kernel(const float* depth, long long hw, float* out
     out[blockIdx.x] = __fmul_rn(m, 1.1f);                                   // torch.max(depth) * 1.1 (Mesher.py:179)
   }
 }
-// The projection of point_masks (Mesher.py:131-150) and cull_mesh.py (:51-67) in float32: T = rows 0-2 of a row-major w2c (12 floats
-// used); cam = T [p, 1]; cam.x = -cam.x; uv = K cam; z = uv.z + eps; inside iff 0 < uv.x/z < W, 0 < uv.y/z < H, z < 0.  cull_mesh.py
-// tests 0 <= -z: at z = +-0 the divisions give inf or NaN, which fail the u test, so z < 0 decides the same.  cam_z = cam.z.
-__device__ __forceinline__ bool in_frustum(const float* T, const float p[3], float fx, float fy, float cx, float cy, float H, float W,
-                                           float eps, float& cam_z) {
-  float c[3];
-  for (int r = 0; r < 3; r++)                                               // w2c @ [p, 1]
-    c[r] = __fmaf_rn(T[4 * r + 3], 1.0f, __fmaf_rn(T[4 * r + 2], p[2], __fmaf_rn(T[4 * r + 1], p[1], __fmul_rn(T[4 * r], p[0]))));
-  c[0] = -c[0];                                                             // cam_cord[:, 0] *= -1
-  const float u0 = __fmaf_rn(cx, c[2], __fmul_rn(fx, c[0]));               // K @ cam (zero entries add nothing)
-  const float v0 = __fmaf_rn(cy, c[2], __fmul_rn(fy, c[1]));
-  const float z = __fadd_rn(c[2], eps);
-  const float u = __fdiv_rn(u0, z), vv = __fdiv_rn(v0, z);
-  cam_z = c[2];
-  return u < W && u > 0.0f && vv < H && vv > 0.0f && z < 0.0f;
-}
+// in_frustum (nsb_geom.cuh) is the projection of point_masks and cull_mesh.py
 __global__ void seen_kernel(const double* verts, int n, const float* w2c, int M, const float* lim, float fx, float fy, float cx, float cy,
                             float H, float W, uint8_t* seen) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;

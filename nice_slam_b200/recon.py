@@ -1,5 +1,6 @@
-"""Reconstruction metrics of a mesh against a ground-truth mesh on the GPU: the 3D metric of the reference's src/tools/eval_recon.py
-(calc_3d_metric, :91-117, with get_align_transformation, :45-59), which needs trimesh and open3d on the host.
+"""Reconstruction metrics of a mesh against a ground-truth mesh on the GPU: the 3D and 2D metrics of the reference's
+src/tools/eval_recon.py (calc_3d_metric, :91-117, with get_align_transformation, :45-59; calc_2d_metric, :120-209), which need trimesh
+and open3d on the host.
 
   read_ply           binary little-endian triangle meshes (mesh.write_ply's, trimesh's and open3d's), validated
   read_ply_records   the same files as their header lines and raw records per element; write_ply_records writes them back
@@ -7,9 +8,12 @@
   NearestNeighbours  exact nearest neighbours on a uniform grid (nsb_nn_*), the role of scipy's cKDTree in eval_recon.py
   icp_align          open3d 0.13's registration_icp, point to point (nsb_icp_sums per iteration, the 3x3 SVD on the host)
   eval_recon         accuracy (cm), completion (cm), completion ratio (% under 5 cm)
+  eval_depth_l1      depth L1 (cm) over 1000 seeded interior views that do not see the unseen region (nice_slam_b200.depth: the
+                     sampling box, the views, the depth rasterizer nsb_depth_render)
 
-python -m nice_slam_b200.recon --rec_mesh A.ply --gt_mesh B.ply -3d   prints eval_recon.py's three lines.  The 2D metric (depth L1 over
-1000 views rendered by open3d's visualiser) is not supported.
+python -m nice_slam_b200.recon --rec_mesh A.ply --gt_mesh B.ply -3d -2d   prints eval_recon.py's three lines, then its "Depth L1: " line.
+-2d reads the unseen-region point cloud beside the ground truth (B_pc_unseen.npy, as eval_recon.py:146); without it -2d exits non-zero
+before any GPU work.
 """
 import argparse
 import ctypes as C
@@ -368,22 +372,72 @@ def eval_recon(rec, gt, align=True, n_samples=200000, seed=0, device="cuda"):
                 completion_ratio=float((d_comp < 0.05).double().mean()) * 100, transform=T, fitness=fit, inlier_rmse=rmse, icp_iterations=it)
 
 
+def unseen_path(gt_meshfile):
+    """The unseen-region point cloud shipped beside a culled ground truth: gt_meshfile.replace('.ply', '_pc_unseen.npy') (eval_recon.py:146)."""
+    return gt_meshfile.replace(".ply", "_pc_unseen.npy")
+
+
+def eval_depth_l1(rec, gt, unseen_points, align=True, n_views=1000, seed=0, H=500, W=500, focal=300.0, device="cuda", view_batch=32):
+    """calc_2d_metric (eval_recon.py:120-209) of rec against gt (paths or (vertices, faces) pairs); unseen_points: [N,3] (or a .npy path),
+    the region no view may see -> dict(depth_l1 [cm], view_errors f64 [n_views] in m, c2w f64 [n_views,4,4], transform, candidates,
+    rejected).
+
+    With align, the rec vertices are moved by icp_align to the gt vertices (threshold 0.1), as eval_recon.  The views are
+    depth.sample_views(gt vertices, unseen_points, n_views, seed); each view renders the gt and the aligned rec with depth.render_depth
+    (z_far 20, each mesh's own z_near = depth.default_z_near, the rec's taken after alignment), and its error is the float64 mean of
+    |gt depth - rec depth| over every pixel, a pixel one mesh misses counting the other's full depth.  depth_l1 = 100 x the mean of the
+    view errors.  Views are rendered view_batch at a time; a repeat gives the same bits."""
+    from . import depth as dp
+    dev = torch.device(device)
+    rv, rf = _mesh(rec, "rec")
+    gv, gf = _mesh(gt, "gt")
+    if isinstance(unseen_points, (str, bytes)) or hasattr(unseen_points, "__fspath__"):
+        unseen_points = np.load(unseen_points)
+    unseen = np.asarray(unseen_points, dtype=np.float64)
+    if unseen.size and (unseen.ndim != 2 or unseen.shape[1] != 3 or not np.isfinite(unseen).all()):
+        raise ValueError("eval_depth_l1: unseen_points must be finite [N,3], got shape %s" % (unseen.shape,))
+    T = np.eye(4)
+    if align:
+        T = icp_align(rv, gv, 0.1, device=dev)[0]
+        rv = rv @ T[:3, :3].T + T[:3, 3]
+    cx, cy = W / 2.0 - 0.5, H / 2.0 - 0.5
+    c2w, drawn, rejected = dp.sample_views(gv, unseen.reshape(-1, 3), n_views, seed, H, W, focal, focal, cx, cy, device=dev)
+    zn_g, zn_r = dp.default_z_near(gv), dp.default_z_near(rv)
+    errs = []
+    for p0 in range(0, len(c2w), int(view_batch)):
+        views = c2w[p0:p0 + int(view_batch)]
+        dg = dp.render_depth(gv, gf, views, H, W, focal, focal, cx, cy, zn_g, dp.Z_FAR, dev)
+        dr = dp.render_depth(rv, rf, views, H, W, focal, focal, cx, cy, zn_r, dp.Z_FAR, dev)
+        errs.append(dp.depth_l1(dg, dr).cpu().numpy())
+    errors = np.concatenate(errs) if errs else np.zeros(0)
+    return dict(depth_l1=float(errors.mean()) * 100 if len(errors) else float("nan"), view_errors=errors, c2w=c2w, transform=T,
+                candidates=drawn, rejected=rejected)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="Arguments to evaluate the reconstruction.")
     ap.add_argument("--rec_mesh", type=str, help="reconstructed mesh file path")
     ap.add_argument("--gt_mesh", type=str, help="ground truth mesh file path")
-    ap.add_argument("-2d", "--metric_2d", action="store_true", help="enable 2D metric (not supported)")
+    ap.add_argument("-2d", "--metric_2d", action="store_true",
+                    help="enable 2D metric (depth L1 over 1000 views; needs the gt's unseen-region cloud, <gt_mesh>_pc_unseen.npy)")
     ap.add_argument("-3d", "--metric_3d", action="store_true", help="enable 3D metric")
     a = ap.parse_args(argv)
+    if (a.metric_3d or a.metric_2d) and (not a.rec_mesh or not a.gt_mesh):
+        ap.error("-3d and -2d need --rec_mesh and --gt_mesh")
+    unseen = None
+    if a.metric_2d:                                    # checked before any GPU work, so a missing file costs no 3D run
+        path = unseen_path(a.gt_mesh)
+        if path == a.gt_mesh or not os.path.isfile(path):
+            sys.exit("nice_slam_b200.recon: %s not found; the 2D metric (depth L1) without the ground truth's unseen-region point cloud "
+                     "is not supported" % path)
+        unseen = np.load(path)
     if a.metric_3d:
-        if not a.rec_mesh or not a.gt_mesh:
-            ap.error("-3d needs --rec_mesh and --gt_mesh")
         r = eval_recon(a.rec_mesh, a.gt_mesh)
         print("accuracy: ", r["accuracy"])
         print("completion: ", r["completion"])
         print("completion ratio: ", r["completion_ratio"])
     if a.metric_2d:
-        sys.exit("nice_slam_b200.recon: the 2D metric (calc_2d_metric: depth L1 over 1000 views rendered by open3d) is not supported")
+        print("Depth L1: ", eval_depth_l1(a.rec_mesh, a.gt_mesh, unseen)["depth_l1"])
 
 
 if __name__ == "__main__":
