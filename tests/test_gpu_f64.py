@@ -11,8 +11,6 @@ The kernels' saved ReLU bits are checked against the sign of the float64 pre-act
 (|u| <= TAU x that layer's largest |u|), and there must be few.
 
 Run with `-s` to print the measured pairs ("f64 <case> <tensor> kernel <4 metrics> port <4 metrics>").  Bars from an H100 run (see DESIGN.md §2)."""
-import os
-
 import pytest
 import torch
 
@@ -39,6 +37,7 @@ K_FP32_PASS = {"max": 10.0, "l2": 10.0, "pe_max": 12.0, "pe_999": 12.0}
 FLOOR = {"max": 1e-7, "l2": 1e-7, "pe_max": 1e-6, "pe_999": 1e-6}
 BIAS_BAR = 8e-7     # measured fwd_f16 scale bias: occupancy -2.1e-7, colour -5.0e-7 (float32 port: 1.7e-8, 2.0e-9)
 TAU = 1e-5          # measured worst flip: |u| = 3.6e-6 x the layer's largest |u|
+TAU_OWN = 4e-6      # knife edge of a kernel without saved ReLU words: just above that worst flip
 
 
 def _option(name, value):
@@ -47,21 +46,20 @@ def _option(name, value):
 
 
 class options:
-    """Library options for the duration of a block, restored afterwards to what the library was loaded with (the NSB_* environment
-    variables nice_slam_b200._lib applies, else the built-in defaults)."""
-    LOADED = {"fwd_f16": int(os.environ.get("NSB_FWD_F16", 0)), "wgrad_tc": int(os.environ.get("NSB_WGRAD_TC", 1)),
-              "split_model": int(os.environ.get("NSB_SPLIT_MODEL", 1)), "pdl": int(os.environ.get("NSB_PDL", 0))}
+    """Library options for the duration of a block, restored afterwards to the values they had on entry (nsb_get_option)."""
 
     def __init__(self, **kw):
         self.kw = kw
 
     def __enter__(self):
+        from nice_slam_b200 import _lib
+        self.saved = {k: _lib.get_option(k) for k in self.kw}
         for k, v in self.kw.items():
             _option(k, v)
 
     def __exit__(self, *exc):
-        for k in self.kw:
-            _option(k, self.LOADED[k])
+        for k, v in self.saved.items():
+            _option(k, v)
 
 
 def cotangents(n, seed):
@@ -141,16 +139,36 @@ def check_masks(label, kern_masks, pre, inb, tau=TAU):
            ["%s: %d mask flips > %d" % (label, n, limit)] * (n > limit)
 
 
+def without_knife_edge_rays(label, grids, dec_state, ro, rd, stage, gd, bound, cot, n_samples, n_surface, coarse_enlarge):
+    """The cotangents with those of the rays zeroed that have an in-bound sample at a ReLU knife edge (|u| <= TAU_OWN x the unit's largest
+    |u|).  A kernel that saves no ReLU words decides every unit on its own float32 pre-activation, which the float64 truth cannot follow; at
+    a knife edge the two may decide differently, and that sample's gradient then differs by the unit's whole share (one such sample set a
+    ray's d_rays_o 7e-2 off, per element, at N = 100, middle stage).  With a zero cotangent such a ray adds nothing to any gradient; its
+    forward outputs are still compared."""
+    t = fr.run(grids, dec_state, ro, rd, stage, gd, bound, *cot, n_samples=n_samples, n_surface=n_surface, coarse_enlarge=coarse_enlarge)
+    pre, inb = t["pre"], t["fixed"]["inb"]
+    scale = pre[inb].abs().amax(0, keepdim=True)
+    knife = ((pre.abs() <= TAU_OWN * scale).flatten(1).any(1) & inb).reshape(ro.shape[0], -1).any(1)
+    print("f64 %-28s %d of %d rays at a knife edge get no cotangent" % (label, int(knife.sum()), knife.numel()))
+    return tuple(torch.where(knife.reshape((-1,) + (1,) * (x.dim() - 1)), torch.zeros_like(x), x) for x in cot)
+
+
 def check_case(label, sc, grids, dec_state, stage, ro, rd, gd, grad_grids=(), grad_decoders=(), n_samples=None, n_surface=None, seed=0,
-               k_bar=None, tau=TAU, opts=None, truth_on_saved_masks=True):
+               k_bar=None, tau=TAU, opts=None, truth_on_saved_masks=True, saved_masks=True, channels_last=True):
+    """saved_masks = False: the forward saves no ReLU words (the FP32-FMA kernels), so the truth is taken on its own signs, the rays with
+    a sample at a knife edge get no cotangent (without_knife_edge_rays) and there are no mask bits to check."""
     k_bar = k_bar or (K_COARSE if stage == "coarse" else K)
     n_samples = sc["rendering"]["N_samples"] if n_samples is None else n_samples
     n_surface = sc["rendering"]["N_surface"] if n_surface is None else n_surface
     bound = su.scene_bound(sc)
     cot = cotangents(ro.shape[0], seed)
-    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, n_samples=n_samples, n_surface=n_surface)
+    if not saved_masks:
+        cot = without_knife_edge_rays(label, grids, dec_state, ro, rd, stage, gd if stage != "coarse" else None, bound, cot, n_samples,
+                                      n_surface, sc["coarse_bound_enlarge"])
+    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, channels_last=channels_last, n_samples=n_samples, n_surface=n_surface)
     with options(**(opts or {})):
         kern = kernel_run(renderer, c, dec, ro, rd, gd, stage, cot, grad_grids, grad_decoders)
+    truth_on_saved_masks = truth_on_saved_masks and saved_masks
     gdp = gd if stage != "coarse" else None
     args = (grids, dec_state, ro, rd, stage, gdp, bound) + cot
     kw = dict(grad_grids=grad_grids, grad_decoders=grad_decoders, n_samples=n_samples, n_surface=n_surface)
@@ -160,7 +178,8 @@ def check_case(label, sc, grids, dec_state, stage, ro, rd, gd, grad_grids=(), gr
     assert torch.equal(kern["z_vals"], tk["z_vals"])
     assert bool((kern["raw"][..., 3][~tk["fixed"]["inb"].reshape(kern["raw"].shape[:2])] == 100).all())
     failures = yardstick(label, kern, tk, port, tpt, stage, k_bar)
-    failures += check_masks(label, kern["masks"], tk["pre"], tk["fixed"]["inb"], tau)
+    if saved_masks:
+        failures += check_masks(label, kern["masks"], tk["pre"], tk["fixed"]["inb"], tau)
     assert not failures, "\n".join(failures)
 
 
@@ -293,9 +312,9 @@ def test_fp16_split_forward_has_no_scale_bias():
 
 
 # ------------------------------------------------------------------------------------ points mode
-@pytest.mark.parametrize("n_points", [256, 129, 191, 192, 193, 255])
-def test_eval_points_against_f64(n_points):
-    """FusedRenderer.eval_points (points mode, one sample per 'ray'): point counts with residues 0, 1, 63, 64, 65, 127 mod 128."""
+def check_points(label, n_points, k_bar=K, k_bar_coarse=K_COARSE, opts=None):
+    """FusedRenderer.eval_points at n_points points in and around the bound (seeded by n_points), coarse and colour stages, against
+    fr.eval_points beside the float32 port."""
     sc, grids, dec_state = scene()
     renderer, c, dec = make_renderer(sc, grids, dec_state, DEV)
     bound = su.scene_bound(sc)
@@ -304,7 +323,8 @@ def test_eval_points_against_f64(n_points):
     p = lo + (hi - lo) * torch.rand(n_points, 3, generator=g, dtype=torch.float64)
     failures = []
     for stage in ("coarse", "color"):
-        got = renderer.eval_points(p.to(DEV), dec, c, stage, DEV).cpu()
+        with options(**(opts or {})):
+            got = renderer.eval_points(p.to(DEV), dec, c, stage, DEV).cpu()
         port = tp.eval_points(p, grids, dec_state, stage, bound)
         t = fr.eval_points(p, grids, dec_state, stage, bound, sc["coarse_bound_enlarge"])
         inb = tp.in_bound_mask(p, bound)
@@ -313,11 +333,17 @@ def test_eval_points_against_f64(n_points):
             if stage == "coarse" and name == "rgb":
                 continue
             ek, ep = fr.errors(got[sel], t[sel]), fr.errors(port[sel], t[sel])
-            print("f64 %-28s %-26s kernel %s port %s" % ("points n=%d %s" % (n_points, stage), name, " ".join("%.1e" % ek[m] for m in METRICS),
+            print("f64 %-28s %-26s kernel %s port %s" % ("%s n=%d %s" % (label, n_points, stage), name, " ".join("%.1e" % ek[m] for m in METRICS),
                                                          " ".join("%.1e" % ep[m] for m in METRICS)))
-            kb = K_COARSE if stage == "coarse" else K
+            kb = k_bar_coarse if stage == "coarse" else k_bar
             failures += ["%s %s %s %s" % (stage, name, m, ek[m]) for m in METRICS if not ek[m] <= kb[m] * ep[m] + FLOOR[m]]
     assert not failures, failures
+
+
+@pytest.mark.parametrize("n_points", [256, 129, 191, 192, 193, 255])
+def test_eval_points_against_f64(n_points):
+    """FusedRenderer.eval_points (points mode, one sample per 'ray'): point counts with residues 0, 1, 63, 64, 65, 127 mod 128."""
+    check_points("points", n_points)
 
 
 # ------------------------------------------------------------------------------------ option pdl

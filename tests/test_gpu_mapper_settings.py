@@ -228,8 +228,8 @@ def test_fine_decoder_weight_gradients_fp32_pass_against_f64(variant, scale, sta
 def test_fine_decoder_weight_gradients_take_the_tensor_core_kernel(stage):
     """Profiler: a mapping iteration with the fine decoder's weight gradients (stage fine: fine; stage color: fine + colour) launches
     render_bwd_wg_tile_kernel and not the FP32-FMA render_bwd_kernel; with wgrad_tc = 0 the reverse."""
-    from torch.profiler import ProfilerActivity, profile
     from nice_slam_b200.steps import IterationContext
+    from test_gpu_wgrad_all import _profiled
     sc, grids, dec_state = scene()
     renderer, c, dec = make_renderer(sc, grids, dec_state, DEV)
     ro, rd, gd, gc = (t.to(DEV) for t in su.make_rays(sc, 200, seed=1500))
@@ -237,11 +237,6 @@ def test_fine_decoder_weight_gradients_take_the_tensor_core_kernel(stage):
     assert ctx.acts is not None and ctx.acts.shape[0] == len(CASES[stage])
     for tc, want, not_want in ((1, "render_bwd_wg_tile_kernel", "render_bwd_kernel"), (0, "render_bwd_kernel", "render_bwd_wg_tile_kernel")):
         with options(wgrad_tc=tc):
-            ctx.run(c, dec, ro, rd, gd, gc.float())
-            torch.cuda.synchronize()
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                ctx.run(c, dec, ro, rd, gd, gc.float())
-                torch.cuda.synchronize()
-        names = [e.name for e in prof.events() if e.device_type.name == "CUDA"]
-        assert any(want in nm for nm in names), (tc, names)
-        assert not any(nm.split("(")[0].split("::")[-1].split("<")[0] == not_want for nm in names), (tc, names)
+            names = _profiled(lambda: ctx.run(c, dec, ro, rd, gd, gc.float()))
+        assert want in names, (tc, names)
+        assert not_want not in names, (tc, names)
