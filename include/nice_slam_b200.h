@@ -82,7 +82,13 @@ const char* nsb_last_error(void);
  * kernels, 3 = tensor-core tile kernels (wgmma 3xTF32, two CTAs per SM).  "split_model": 1 (default) = a tile's decoders are spread over CTAs only while
  * that beats one CTA per tile by wave efficiency, 0 = always for batches of <= 262144 points.  "wgrad_all": 0 (default) = only fine / colour
  * decoder weight gradients take the tensor cores, 1 = any decoders' (middle and coarse too) whose layer outputs the forward kept
- * (nsb_forward_outputs.acts_levels may then name them).  "wgrad_tc", "fwd_f16", "pdl", "small_rays": DESIGN.md. */
+ * (nsb_forward_outputs.acts_levels may then name them).  "wgrad_tc", "fwd_f16", "pdl", "small_rays": DESIGN.md.
+ * "deterministic": 0 (default), 1 = the backward's voxel and decoder-weight gradients are summed in an order fixed by the data (nsb_voxel_grad_ordered
+ * and a tile-ordered sum of per-tile weight-gradient images) instead of by float atomics in CTA order, so that the same build on the same GPU
+ * model gives the same bits for the same inputs (INTEGRATION.md).  It implies wgrad_all; nsb_split_workspace_bytes and
+ * nsb_iteration_workspace_bytes then include its buffers (a workspace sized with the option off is refused, NSB_ERR_ARG).  Refused together
+ * with mlp_backend 1 or 2 or wgrad_tc 0 (NSB_ERR_ARG, whichever is set second), and by a backward that would need the FP32-FMA kernels or the
+ * sharded tail for its voxel / weight gradients (NSB_ERR_UNSUPPORTED). */
 int nsb_set_option(const char* key, int value);
 /* Current value of an option of nsb_set_option -> *value (NSB_ERR_ARG for an unknown key). */
 int nsb_get_option(const char* key, int* value);
@@ -255,6 +261,16 @@ int nsb_masked_gather(const nsb_grid* grid, const int32_t* slot_map, float* comp
 int nsb_masked_scatter(const nsb_grid* grid, const int32_t* slot_map, const float* compact, void* stream); /* val[mask] = compact */
 /* to_reference != 0: [n][32] -> [32][n] (the reference's val[mask] order); 0: the inverse. */
 int nsb_compact_transpose(const float* src, float* dst, long long n_selected, int to_reference, void* stream);
+
+/* The voxel-gradient sum of option "deterministic": for n_points points with normalised coordinates xn f32 [n][3] (grid_sample's, in [-1, 1]
+ * inside the bound) and dL/dc f32 [n][32], every corner k (bit 0 +x, bit 1 +y, bit 2 +z) of point p's trilinear cell that lies inside the grid
+ * adds fl(w_k * dc[p][c]) -- w_k the float32 trilinear weight of the backward's scatter, border-clipped -- to channel c of its voxel:
+ * d_grid dense with grid->strides (slot_map NULL) or the compact [n_selected][32] buffer at slot_map[voxel] (slot -1: skipped).  The
+ * contributions to one voxel channel are added one by one in ascending (p, k) order, in float32, to d_grid's current value.  grid->data is not
+ * read.  workspace: nsb_voxel_grad_ordered_workspace(n_points) bytes, 16-byte aligned; n_points < 2^28, D*H*W < 2^32 - 1. */
+size_t nsb_voxel_grad_ordered_workspace(int n_points);
+int nsb_voxel_grad_ordered(const nsb_grid* grid, const int32_t* slot_map, const float* xn, const float* dc, int n_points, float* d_grid,
+                           void* workspace, size_t workspace_bytes, void* stream);
 
 /* Fused Adam steps (torch.optim.Adam with its defaults -- no weight decay, no amsgrad -- as the mapper uses it, src/Mapper.py:365-379,
  * per-group learning rates set per stage :412-419, step :504), float32 arithmetic in torch's operation order.  `step` = 1-based count of

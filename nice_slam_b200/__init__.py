@@ -13,9 +13,9 @@ Public surface:
     build_scene     NICE_SLAM.__init__'s initial state (bound, grids, pretrained decoders, renderer) from a config (scene.py)
     FrameReader     the reference's dataset readers, frames prepared on the GPU (datasets.py)
     run             run.py's counterpart: python -m nice_slam_b200.run CONFIG (not imported here)
-    to_channels_last, lib (ctypes handle of libnsb.so)
+    to_channels_last, lib (ctypes handle of libnsb.so), get_option / set_option (library options, e.g. "deterministic")
 """
-from ._lib import lib, LIB_PATH                       # noqa: F401
+from ._lib import lib, LIB_PATH, get_option, set_option   # noqa: F401
 from .decoders import NICEDecoders                     # noqa: F401
 from .renderer import FusedRenderer, to_channels_last  # noqa: F401
 from .mapping import FusedMapper                       # noqa: F401
@@ -24,4 +24,4 @@ from .slam import FusedSLAM, ate_rmse                  # noqa: F401
 from .scene import build_scene                         # noqa: F401
 from .datasets import FrameReader                      # noqa: F401
 
-__all__ = ["FusedRenderer", "FusedMapper", "FusedSLAM", "FusedMesher", "ate_rmse", "build_scene", "FrameReader", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH"]
+__all__ = ["FusedRenderer", "FusedMapper", "FusedSLAM", "FusedMesher", "ate_rmse", "build_scene", "FrameReader", "NICEDecoders", "to_channels_last", "lib", "LIB_PATH", "get_option", "set_option"]

@@ -128,6 +128,8 @@ SYMBOLS = {
     "nsb_masked_gather": (C.c_int, [C.POINTER(Grid), _P, _P, _P]),
     "nsb_masked_scatter": (C.c_int, [C.POINTER(Grid), _P, _P, _P]),
     "nsb_compact_transpose": (C.c_int, [_P, _P, C.c_longlong, C.c_int, _P]),
+    "nsb_voxel_grad_ordered_workspace": (C.c_size_t, [C.c_int]),
+    "nsb_voxel_grad_ordered": (C.c_int, [C.POINTER(Grid), _P, _P, _P, C.c_int, _P, _P, C.c_size_t, _P]),
     "nsb_pose_grad_frames": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P]),
     "nsb_split_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nsb_adam_masked_voxels": (C.c_int, [C.POINTER(Grid), _P, _P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, _P]),
@@ -228,6 +230,9 @@ def lib():
         sm = os.environ.get("NSB_SPLIT_MODEL")               # 0 = per-decoder items for every batch of <= 262144 points (default: by wave efficiency)
         if sm is not None:
             h.nsb_set_option(b"split_model", int(sm))
+        det = os.environ.get("NSB_DETERMINISTIC")            # 1 = voxel and decoder-weight gradients summed in a fixed order (default: 0)
+        if det is not None and h.nsb_set_option(b"deterministic", int(det)) != 0:
+            raise RuntimeError("NSB_DETERMINISTIC=%r: %s" % (det, h.nsb_last_error().decode("utf-8", "replace")))
         _LIB = h
     return _LIB
 
@@ -243,6 +248,12 @@ def get_option(name):
     v = C.c_int(0)
     check(lib().nsb_get_option(name.encode(), C.byref(v)), "nsb_get_option(%s)" % name)
     return v.value
+
+
+def set_option(name, value):
+    """Set a library option (nsb_set_option); raises with the library's message when it refuses.  Workspaces sized before a change of
+    option "deterministic" do not fit the new mode: build fused contexts after setting it."""
+    check(lib().nsb_set_option(name.encode(), int(value)), "nsb_set_option(%s)" % name)
 
 
 def flat_layout(level):

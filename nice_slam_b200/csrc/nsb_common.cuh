@@ -222,6 +222,14 @@ int make_peerx(const struct nsb_peers* p, PeerX* px);
 int eval_points_mesh(const nsb_render_inputs* in, const double* points, const nsb_mesh_lattice* lat, int n_points, float* raw, float* z,
                      void* stream);
 
+// deterministic mode (option "deterministic", nsb_det.cu): the ordered voxel-gradient reduction over n_points points' normalised coordinates
+// xn [n][3] and dL/dc [n][32] into d_grid (dense with g's strides, or compact through slot_map), and the tile-ordered sum of per-tile partial
+// images part [tiles][n_floats] -> out
+size_t det_voxel_workspace_bytes(long long n_points);
+int det_voxel_reduce(const nsb_grid& g, const int32_t* slot_map, const float* xn, const float* dc, long long n_points, float* d_grid,
+                     void* workspace, size_t workspace_bytes, cudaStream_t st);
+int det_tile_sum(const float* part, int tiles, int n_floats, float* out, cudaStream_t st);
+
 // error plumbing shared by the API translation units
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);

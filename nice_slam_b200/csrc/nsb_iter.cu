@@ -23,7 +23,12 @@ static int check_buffers(const nsb_render_inputs* in, const nsb_iteration_buffer
   if (!in || !b || !g) { set_error("iteration: NULL argument"); return NSB_ERR_ARG; }
   if (!b->depth || !b->var || !b->rgb || !b->z_vals || !b->raw || !b->g_depth || !b->g_rgb || !b->loss || !b->depth_max || !b->workspace) {
     set_error("iteration: incomplete nsb_iteration_buffers"); return NSB_ERR_ARG; }
-  if (b->workspace_bytes < nsb_iteration_workspace_bytes(in->n_rays)) { set_error("iteration: workspace too small"); return NSB_ERR_ARG; }
+  if (b->workspace_bytes < nsb_iteration_workspace_bytes(in->n_rays)) {
+    int det = 0; nsb_get_option("deterministic", &det);
+    set_error(det ? "iteration: workspace smaller than nsb_iteration_workspace_bytes(%d) with option deterministic on (size it after setting the option)"
+                  : "iteration: workspace too small", in->n_rays);
+    return NSB_ERR_ARG;
+  }
   return NSB_OK;
 }
 

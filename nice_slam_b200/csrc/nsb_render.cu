@@ -178,6 +178,11 @@ struct KParams {
 // (Mesher.get_grid_uniform, Mesher.py:334-345); the in-bound test is Mesher.eval_points' float32 one (Mesher.py:301-304), and a point
 // outside the hull's half-spaces counts as out of bound (z = 100, Mesher.py:433); lattice occupancies go to z [P] instead of raw.
 struct MeshPoints { nsb_mesh_lattice lat; int lattice; float* z; };
+// Deterministic mode (option "deterministic") runs the tile backward with this second parameter block (the default kernels do not carry it):
+// instead of adding into the voxel and weight gradients, the items write per level l the dL/dc rows dc[l] [N*S][32] and the normalised
+// coordinates xn[l] [N*S][3] of their points (when bw.d_grid[l] is set), and the weight-gradient image of decoder l of tile t to
+// wpart[l] + t * packed_floats(l) (zeroed by the host); nsb_det.cu sums both in a fixed order.
+struct DetParams { float* dc[4]; float* xn[4]; float* wpart[4]; };
 __device__ __forceinline__ double lattice_value(const nsb_mesh_lattice& L, int a, int i) {
   return i == L.n[a] - 1 ? L.stop[a] : __dadd_rn(__dmul_rn((double)i, L.step[a]), L.start[a]);
 }
@@ -1105,15 +1110,16 @@ static int weight_bytes(const int* dec, int n) {
 }
 
 static int g_wgrad_all = 0;        // weight gradients of every decoder (middle and coarse too) on the tensor cores when the forward kept their layer outputs
+static int g_deterministic = 0;    // voxel and weight gradients summed in a fixed order (nsb_det.cu); implies wgrad_all
 
 // nsb_forward_outputs / nsb_backward_args .acts_levels -> K.acts_mask (0 keeps fill_common's default): the fine and colour decoders of the stage,
 // with option wgrad_all any decoder of the stage
 static int apply_acts_levels(KParams& K, int levels) {
   if (levels == 0) return NSB_OK;
   int stage_mask = 0; for (int i = 0; i < K.n_dec; i++) stage_mask |= 1 << K.dec[i];
-  const int allowed = g_wgrad_all ? 0xf : (1 << NSB_FINE) | (1 << NSB_COLOR);
+  const int allowed = (g_wgrad_all || g_deterministic) ? 0xf : (1 << NSB_FINE) | (1 << NSB_COLOR);
   if ((levels & ~allowed) || (levels & ~stage_mask)) {
-    set_error(g_wgrad_all ? "acts_levels 0x%x: only decoders of the stage keep layer outputs"
+    set_error((g_wgrad_all || g_deterministic) ? "acts_levels 0x%x: only decoders of the stage keep layer outputs"
                           : "acts_levels 0x%x: only the fine / colour decoders of the stage keep layer outputs (middle / coarse: option wgrad_all)",
               levels);
     return NSB_ERR_ARG;
@@ -1234,8 +1240,29 @@ static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd, int ctas_p
   else K.tile_parts = split > 1 ? static_cast<float4*>(ws) : reinterpret_cast<float4*>(K.fo.raw);
   return NSB_OK;
 }
-extern "C" size_t nsb_split_workspace_bytes(int n_rays, int S) {
-  if (n_rays < 1 || S < 1) return 0;
+// Deterministic mode's share of the split workspace, placed right above the largest per-item scratch a batch of N rays can use (split_scratch_bytes,
+// monotone in N, like the region itself: a buffer sized for a capacity keeps it clear of the ray counters of every batch up to that
+// capacity, which sit at the END of the buffer and must stay zero between calls): per stage decoder (up to three) dL/dc [N*S][32] and
+// coordinates [N*S][3] of its points, per-tile weight-gradient images of the stage's decoders (the middle, fine and colour decoders' at most),
+// and the sort of the ordered voxel reduction (reused grid after grid).
+struct DetWs { float* dc[3]; float* xn[3]; float* wpart[3]; void* sort; size_t sort_bytes; };
+static size_t det_ws_bytes(int N, int S, DetWs* w = nullptr, char* base = nullptr) {
+  const long long NP = (long long)N * S, tiles = tile_count(NP);
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t r = o; o = align16(o + bytes); return r; };
+  size_t o_dc[3], o_xn[3], o_wp[3];
+  for (int i = 0; i < 3; i++) o_dc[i] = take((size_t)NP * 32 * 4);
+  for (int i = 0; i < 3; i++) o_xn[i] = take((size_t)NP * 3 * 4);
+  for (int i = 0; i < 3; i++) o_wp[i] = take((size_t)tiles * packed_floats(i + 1) * 4);      // (>= the coarse decoder's alone)
+  const size_t sb = det_voxel_workspace_bytes(NP), o_s = take(sb);
+  if (w != nullptr) {
+    for (int i = 0; i < 3; i++) { w->dc[i] = (float*)(base + o_dc[i]); w->xn[i] = (float*)(base + o_xn[i]); w->wpart[i] = (float*)(base + o_wp[i]); }
+    w->sort = base + o_s; w->sort_bytes = sb;
+  }
+  return o;
+}
+// per-item scratch of the tile kernels that nsb_split_workspace_bytes reserves at the start of the buffer (S >= NSB_MAX_SAMPLES: for any S)
+static size_t split_scratch_bytes(int n_rays, int S) {
   auto need_exact = [&](int n, int s) {
     const int split = (long long)n * s <= kSplitMaxPts ? 3 : 1;
     const size_t a = tile_scratch_bytes(n, s, split, false), b = tile_scratch_bytes(n, s, split, true);
@@ -1248,7 +1275,13 @@ extern "C" size_t nsb_split_workspace_bytes(int n_rays, int S) {
   };
   size_t m = need(S);
   if (S >= NSB_MAX_SAMPLES) for (int s = tl::kMinSamples; s < NSB_MAX_SAMPLES; s++) { const size_t v = need(s); if (v > m) m = v; }   // "any S" sizing (nsb_iteration_workspace_bytes)
+  return m;
+}
+extern "C" size_t nsb_split_workspace_bytes(int n_rays, int S) {
+  if (n_rays < 1 || S < 1) return 0;
+  size_t m = split_scratch_bytes(n_rays, S);
   m += 16 + align16((size_t)n_rays * sizeof(int));
+  if (g_deterministic) m += det_ws_bytes(n_rays, S < NSB_MAX_SAMPLES ? S : NSB_MAX_SAMPLES);
   const size_t old = old_split_workspace_bytes(n_rays, S);
   return m > old ? m : old;
 }
@@ -1289,7 +1322,7 @@ enum class Family { Tile, Group, Fma };
 static Family kernel_family(int S, int n_rays, bool points) {
   const bool tile_backend = g_mlp_backend == 0 || g_mlp_backend == 3;
   if (points) return tile_backend ? Family::Tile : g_mlp_backend == 2 ? Family::Group : Family::Fma;
-  const bool small = g_mlp_backend == 0 && n_rays <= g_small_rays && S <= kMaxPtsTc;
+  const bool small = g_mlp_backend == 0 && n_rays <= g_small_rays && S <= kMaxPtsTc && !g_deterministic;
   if (tile_backend && S >= tl::kMinSamples && S <= NSB_MAX_SAMPLES && !small) return Family::Tile;
   if ((g_mlp_backend == 0 || g_mlp_backend == 2) && S <= kMaxPtsTc) return Family::Group;
   return Family::Fma;
@@ -1312,6 +1345,9 @@ static int set_attrs() {
     {(const void*)render_bwd_tile_kernel, tile_smem_bytes(true), true, "render_bwd_tile_kernel"},
     {(const void*)render_bwd_wg_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_tile_kernel"},
     {(const void*)render_bwd_wg_coarse_tile_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_coarse_tile_kernel"},
+    {(const void*)render_bwd_tile_det_kernel, tile_smem_bytes(true), true, "render_bwd_tile_det_kernel"},
+    {(const void*)render_bwd_wg_tile_det_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_tile_det_kernel"},
+    {(const void*)render_bwd_wg_coarse_tile_det_kernel, tile_wg_smem_bytes(), false, "render_bwd_wg_coarse_tile_det_kernel"},
   };
   for (const auto& a : attrs)
     if (check_cuda(cudaFuncSetAttribute(a.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)a.smem), a.name) ||
@@ -1363,21 +1399,31 @@ static int launch_fma(KParams K, bool bwd, cudaStream_t st) {
 
 using namespace nsb;
 
+// Option combinations deterministic mode cannot honour: the FP32-FMA and round-1 ray-group back-ends and the FP32-FMA weight-gradient pass add
+// their gradients with atomics in CTA order.
+static bool det_conflict(int det, int backend, int wgrad_tc) {
+  if (!det) return false;
+  if (backend == 1 || backend == 2) { set_error("option deterministic needs mlp_backend 0 or 3 (got mlp_backend %d)", backend); return true; }
+  if (!wgrad_tc) { set_error("option deterministic needs wgrad_tc = 1 (got wgrad_tc 0)"); return true; }
+  return false;
+}
 extern "C" int nsb_set_option(const char* key, int value) {
-  if (key && !strcmp(key, "wgrad_tc")) { g_wgrad_tc = value != 0; return NSB_OK; }
+  if (key && !strcmp(key, "deterministic")) { if (det_conflict(value != 0, g_mlp_backend, g_wgrad_tc)) return NSB_ERR_ARG; g_deterministic = value != 0; return NSB_OK; }
+  if (key && !strcmp(key, "wgrad_tc")) { if (det_conflict(g_deterministic, g_mlp_backend, value != 0)) return NSB_ERR_ARG; g_wgrad_tc = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "wgrad_all")) { g_wgrad_all = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "fwd_f16")) { g_fwd_f16 = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "pdl")) { g_pdl = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "split_model")) { g_split_model = value != 0; return NSB_OK; }
   if (key && !strcmp(key, "small_rays")) { if (value < 0) { set_error("small_rays must be >= 0"); return NSB_ERR_ARG; } g_small_rays = value; return NSB_OK; }
-  if (key && !strcmp(key, "mlp_backend")) { if (value < 0 || value > 3) { set_error("mlp_backend must be 0 (auto = tile kernels), 1 (FP32-FMA), 2 (round-1 ray-group tensor-core kernels) or 3 (tensor-core tile kernels)"); return NSB_ERR_ARG; } g_mlp_backend = value; return NSB_OK; }
+  if (key && !strcmp(key, "mlp_backend")) { if (det_conflict(g_deterministic, value, g_wgrad_tc)) return NSB_ERR_ARG; if (value < 0 || value > 3) { set_error("mlp_backend must be 0 (auto = tile kernels), 1 (FP32-FMA), 2 (round-1 ray-group tensor-core kernels) or 3 (tensor-core tile kernels)"); return NSB_ERR_ARG; } g_mlp_backend = value; return NSB_OK; }
   set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
 }
 
 extern "C" int nsb_get_option(const char* key, int* value) {
   if (!value) { set_error("nsb_get_option: value is NULL"); return NSB_ERR_ARG; }
   const struct { const char* name; int v; } opts[] = {{"wgrad_tc", g_wgrad_tc}, {"wgrad_all", g_wgrad_all}, {"fwd_f16", g_fwd_f16}, {"pdl", g_pdl},
-                                                      {"split_model", g_split_model}, {"small_rays", g_small_rays}, {"mlp_backend", g_mlp_backend}};
+                                                      {"split_model", g_split_model}, {"small_rays", g_small_rays}, {"mlp_backend", g_mlp_backend},
+                                                      {"deterministic", g_deterministic}};
   for (const auto& o : opts)
     if (key && !strcmp(key, o.name)) { *value = o.v; return NSB_OK; }
   set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
@@ -1545,7 +1591,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     if (ig.n_dec > 0) { L[n] = ig; kind[n++] = fam == Family::Tile ? TileIg : GroupIg; }
     bool wg_tc = wg.n_dec > 0 && bw->acts != nullptr && fam == Family::Tile && g_wgrad_tc && !sharded;
     for (int i = 0; i < wg.n_dec; i++)
-      wg_tc = wg_tc && (g_wgrad_all || wg.dec[i] == NSB_FINE || wg.dec[i] == NSB_COLOR) && ((K.acts_mask >> wg.dec[i]) & 1);
+      wg_tc = wg_tc && (g_wgrad_all || g_deterministic || wg.dec[i] == NSB_FINE || wg.dec[i] == NSB_COLOR) && ((K.acts_mask >> wg.dec[i]) & 1);
     if (wg.n_dec > 0) { L[n] = wg; kind[n++] = wg_tc ? WgTile : Fma; }       // (every decoder here: wg == K)
   }
   // Every launch after the first adds to the ray gradients; the last one writes d c2w from its last CTA (the FP32-FMA kernel does not:
@@ -1556,9 +1602,62 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     if (n > 1 || !want_pose) { set_error("sharded backward tail needs pose_dirs and no decoder weight gradients"); return NSB_ERR_ARG; }
     L[0].tail = *tail;
   }
+  // Deterministic mode: the tile launches that produce voxel or weight gradients take the kDet instantiations, and nsb_det.cu sums what they
+  // leave in the split workspace after the last launch.  Backward calls without those gradients (the tracker's) are order-free already.
+  const long long NP = (long long)in->n_rays * K.S;
+  bool det_grads = any_w;
+  for (int l = 0; l < 4; l++) det_grads |= K.bw.d_grid[l] != nullptr;
+  const bool det = g_deterministic && det_grads;
+  DetWs dw; memset(&dw, 0, sizeof(dw));
+  if (det) {
+    if (sharded) { set_error("option deterministic: the sharded backward tail sums over ranks in arrival order (turn deterministic off)"); return NSB_ERR_UNSUPPORTED; }
+    for (int i = 0; i < n; i++)
+      if (kind[i] != TileIg && kind[i] != WgTile) {
+        set_error("option deterministic: voxel and decoder gradients need the tile backward with the forward's ReLU masks and, for decoder weights, its "
+                  "layer outputs (acts / acts_levels)");
+        return NSB_ERR_UNSUPPORTED;
+      }
+    const size_t room = bw->split_workspace_bytes & ~size_t(15);
+    const size_t base = split_scratch_bytes(in->n_rays, K.S);
+    const size_t need = base + det_ws_bytes(in->n_rays, K.S) + 16 + align16((size_t)in->n_rays * sizeof(int));
+    if (!bw->split_workspace || (reinterpret_cast<uintptr_t>(bw->split_workspace) & 15) || room < need) {
+      set_error("split_workspace smaller than nsb_split_workspace_bytes(%d, %d) with option deterministic on (size it after setting the option)",
+                in->n_rays, K.S);
+      return NSB_ERR_ARG;
+    }
+    det_ws_bytes(in->n_rays, K.S, &dw, static_cast<char*>(bw->split_workspace) + base);
+  }
+  auto det_params = [&](const KParams& P, bool wg) {
+    DetParams D; memset(&D, 0, sizeof(D));
+    for (int j = 0; j < K.n_dec; j++) {
+      const int lv = K.dec[j];
+      bool in_launch = false; for (int q = 0; q < P.n_dec; q++) in_launch |= P.dec[q] == lv;
+      if (!in_launch) continue;
+      if (P.bw.d_grid[lv] != nullptr) { D.dc[lv] = dw.dc[j]; D.xn[lv] = dw.xn[j]; }
+      if (wg) D.wpart[lv] = dw.wpart[lv > 0 ? lv - 1 : 0];
+    }
+    return D;
+  };
   for (int i = 0; i < n; i++) {
     KParams& P = L[i];
     const unsigned tiles = (unsigned)tile_count((long long)in->n_rays * P.S);
+    if (det && (kind[i] == TileIg || kind[i] == WgTile)) {
+      if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true, kind[i] == WgTile ? 1 : 2))) return rc;
+      const DetParams D = det_params(P, kind[i] == WgTile);
+      if (kind[i] == WgTile) {
+        for (int q = 0; q < P.n_dec; q++)
+          if (check_cuda(cudaMemsetAsync(D.wpart[P.dec[q]], 0, (size_t)tiles * packed_floats(P.dec[q]) * 4, st), "memset weight-gradient partials"))
+            return NSB_ERR_CUDA;
+        if (P.dec[0] == NSB_COARSE) render_bwd_wg_coarse_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P, D);
+        else render_bwd_wg_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P, D);
+      } else {
+        render_bwd_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_smem_bytes(true), st>>>(P, D);
+      }
+      if ((rc = check_cuda(cudaGetLastError(), "deterministic tile backward launch"))) return rc;
+      for (int q = 0; q < P.n_dec && kind[i] == WgTile; q++)
+        if ((rc = det_tile_sum(D.wpart[P.dec[q]], (int)tiles, packed_floats(P.dec[q]), K.d_packed[P.dec[q]], st))) return rc;
+      continue;
+    }
     if (kind[i] == GroupIg) rc = launch_group(P, true, bw->split_workspace, bw->split_workspace_bytes, st);
     else if (kind[i] == Fma) rc = launch_fma(P, true, st);
     else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true, kind[i] == WgTile ? 1 : 2))) return rc;
@@ -1584,6 +1683,11 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
       rc = check_cuda(cudaGetLastError(), "render_bwd_tile_kernel launch");
     }
     if (rc) return rc;
+  }
+  for (int j = 0; j < K.n_dec && det; j++) {                      // (stage order; every grid has one sampler with a gradient)
+    const int lv = K.dec[j];
+    if (K.bw.d_grid[lv] != nullptr &&
+        (rc = det_voxel_reduce(in->grid[lv], bw->slot_map[lv], dw.xn[j], dw.dc[j], NP, K.bw.d_grid[lv], dw.sort, dw.sort_bytes, st))) return rc;
   }
   if (any_w && (rc = launch_unpack_grads(K.d_packed, bw->d_flat, st))) return rc;
   if (kind[n - 1] == Fma && want_pose) {

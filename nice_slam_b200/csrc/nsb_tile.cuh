@@ -842,7 +842,10 @@ __device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, in
 // the xyz one took that kernel past 255 registers (spills).
 enum { kWgNone = 0, kWgXyz = 1, kWgCoarse = 2 };
 __device__ __forceinline__ int bwd_dpe_off(int r) { return (r >> 6) * (64 * 32) + (r & 63) * 4; }
-template <int WG>
+// kDet (deterministic mode): the per-warp bias partials are added in warp order through shared memory and stored, not reduced by atomics
+// (w->dpk is then this tile's own zeroed partial image, which every other element of receives exactly one reduction per tile).
+__device__ __forceinline__ float* det_bias_smem() { __shared__ float s[8 * 64]; return s; }
+template <int WG, bool kDet = false>
 __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t, Issuer& I, const BwdExtra& X, int lv, const PointGeom& G, int hb, uint32_t hdr_parity,
                                              const uint32_t* __restrict__ masks, int npts, int off0, long long gp0, WgSmem* w = nullptr, const float* acts_row = nullptr) {
   const int row = threadIdx.x & (TM - 1), cg = threadIdx.x >> 7, warp = threadIdx.x >> 5;
@@ -912,7 +915,19 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
     if (cg == 0) {
       const float sb = warp_colsum16(go, lane);
       const int col = colsum_col(lane);
-      if ((lane & 1) == 0 && col < DW.no) atomicAdd(w->dpk + DW.o_bo + col, sb);
+      if ((lane & 1) == 0 && col < DW.no) {
+        if constexpr (kDet) det_bias_smem()[warp * 64 + col] = sb;
+        else atomicAdd(w->dpk + DW.o_bo + col, sb);
+      }
+    }
+    if constexpr (kDet) {
+      __syncthreads();
+      if ((int)threadIdx.x < DW.no) {
+        float s = 0.0f;
+        for (int wp = 0; wp < 4; wp++) s = __fadd_rn(s, det_bias_smem()[wp * 64 + threadIdx.x]);
+        w->dpk[DW.o_bo + threadIdx.x] = s;
+      }
+      __syncthreads();
     }
   }
 #pragma unroll 1
@@ -939,8 +954,22 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       float sc = 0.0f;
       if constexpr (WG != kWgCoarse) sc = frag_colsum(d1, lane);
       const int col = frag_colsum_col(lane);
-      atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb);
-      if constexpr (WG != kWgCoarse) atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
+      if constexpr (kDet) {
+        float* sbias = det_bias_smem();
+        sbias[warp * 64 + col] = sb;
+        if constexpr (WG != kWgCoarse) sbias[warp * 64 + 32 + col] = sc;
+        __syncthreads();
+        if ((int)threadIdx.x < (WG != kWgCoarse ? 64 : 32)) {
+          const int c = threadIdx.x & 31;
+          float s = 0.0f;
+          for (int wp = 0; wp < kThreads / 32; wp++) s = __fadd_rn(s, sbias[wp * 64 + threadIdx.x]);
+          w->dpk[(threadIdx.x < 32 ? DW.o_b : DW.o_bc) + 32 * i + c] = s;
+        }
+        __syncthreads();
+      } else {
+        atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb);
+        if constexpr (WG != kWgCoarse) atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
+      }
     }
     fence_proxy_async();
     wg_bar_sync();                                               // this warpgroup's rows of G / DU are written -> its MMAs
@@ -1055,9 +1084,11 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
 }
 
 // Backward of gather_tile (same warp -> rows mapping).  dcs = [128][32] fp32.  emit(row, gx) once per point.
-template <typename F>
+// kStore (deterministic mode, dgrid NULL): rows < npts of dcs and their coordinates also go to dc_out [rows][32] / xn_out [rows][3], if non-NULL.
+template <bool kStore = false, typename F>
 __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restrict__ dgrid, const int32_t* __restrict__ slots,
-                                             const float* dcs, const float xn[3], int warp, int lane, F&& emit) {
+                                             const float* dcs, const float xn[3], int warp, int lane, F&& emit,
+                                             float* dc_out = nullptr, float* xn_out = nullptr, int npts = 0) {
   const int q = lane & 7, qd = warp & 3, it0 = (warp >> 2) * 4;
 #pragma unroll 1
   for (int it = it0; it < it0 + 4; it++) {
@@ -1067,6 +1098,12 @@ __device__ __forceinline__ void scatter_tile(const nsb_grid& g, float* __restric
     x[0] = __shfl_sync(0xffffffffu, xn[0], src_lane); x[1] = __shfl_sync(0xffffffffu, xn[1], src_lane); x[2] = __shfl_sync(0xffffffffu, xn[2], src_lane);
     const float4 d4 = *reinterpret_cast<const float4*>(dcs + row * 32 + 4 * q);
     const float dc[4] = {d4.x, d4.y, d4.z, d4.w};
+    if constexpr (kStore) {
+      if (dc_out != nullptr && row < npts) {
+        __stcg(reinterpret_cast<float4*>(dc_out + row * 32 + 4 * q), d4);
+        if (q < 3) xn_out[3 * row + q] = x[q];
+      }
+    }
     float gx[3];
     scatter_pass(g, dgrid, slots, x, dc, q, gx);
     if (q == 0) emit(row, gx);
@@ -1311,8 +1348,10 @@ __global__ void __launch_bounds__(tl::kThreads, 2) render_fwd_tile_mesh_kernel(c
 // WG != kWgNone: the item's decoder also gets its WEIGHT gradients (tensor-core contraction over the tile's points, see the "tensor-core weight
 // gradients" helpers; kWgXyz: the middle, fine and colour decoders, kWgCoarse: the coarse decoder): 96 KB more shared memory in front of the
 // common part -> one CTA per SM.
-template <int WG>
-__device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
+// kDet: the deterministic-mode instantiation (DetParams D): dL/dc rows and coordinates go to D->dc / D->xn instead of the voxel scatter (which
+// still yields the coordinate gradients), weight gradients to this tile's partial image in D->wpart.
+template <int WG, bool kDet = false>
+__device__ __forceinline__ void render_bwd_tile_body(const KParams& P, const DetParams* D = nullptr) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using namespace tl;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1401,21 +1440,25 @@ __device__ __forceinline__ void render_bwd_tile_body(const KParams& P) {
       const uint32_t* gm = P.bw.masks + (gp0 * 15 + P.dec_pos[qd] * 5);
       const int dq = qd - q0;
       if (tid == 0 && qd + 1 < q1) load_header(P, t, P.dec[qd + 1], (dq + 1) & 1);      // (the previous decoder ended with CTA barriers: its buffer is free)
-      if (WG) wg.dpk = P.d_packed[lv];
+      if constexpr (kDet) { if (WG) wg.dpk = D->wpart[lv] + (size_t)tile * packed_floats(lv); }
+      else if (WG) wg.dpk = P.d_packed[lv];
       const float* acts_row = (WG && row < npts) ? P.bw.acts + ((acts_slot(P.acts_mask, lv) * NP + gp0 + row) * 5) * 32 + kCW * cg : nullptr;
-      epi_backward<WG>(P, t, I, X, lv, G, dq & 1, (dq >> 1) & 1u, gm, npts, off0, gp0, WG ? &wg : nullptr, acts_row);
+      epi_backward<WG, kDet>(P, t, I, X, lv, G, dq & 1, (dq >> 1) & 1u, gm, npts, off0, gp0, WG ? &wg : nullptr, acts_row);
       epi_sync();                                                 // dL/dc rows + embedding partials visible
       const double* bb = lv == 0 ? P.in.coarse_bound : P.in.bound;
       const double sc[3] = {2.0 / (bb[1] - bb[0]), 2.0 / (bb[3] - bb[2]), 2.0 / (bb[5] - bb[4])};      // d(normalised)/dp, common.py:280-282
       const float* xn = lv == 0 ? G.xnc : G.xn;
-      scatter_tile(P.in.grid[lv], P.bw.d_grid[lv], P.bw.slot_map[lv], t.a[0], xn, warp, lane, [&](int prow, const float gx[3]) {
+      // (kDet: this tile's rows of dL/dc and coordinates go to D for nsb_det.cu's ordered sum instead of the voxel scatter)
+      float* const dc_out = kDet && D->dc[lv] != nullptr ? D->dc[lv] + gp0 * 32 : nullptr;
+      float* const xn_out = kDet && D->dc[lv] != nullptr ? D->xn[lv] + gp0 * 3 : nullptr;
+      scatter_tile<kDet>(P.in.grid[lv], kDet ? nullptr : P.bw.d_grid[lv], P.bw.slot_map[lv], t.a[0], xn, warp, lane, [&](int prow, const float gx[3]) {
         if (prow < npts) {
           const float4 p = *reinterpret_cast<const float4*>(t.a[1] + bwd_dpe_off(prow));
           const float dpe[3] = {p.x, p.y, p.z};
 #pragma unroll
           for (int a = 0; a < 3; a++) X.dp[3 * prow + a] += (double)dpe[a] + (double)gx[a] * sc[a];
         }
-      });
+      }, dc_out, xn_out, npts);
       epi_sync();                                                 // reads of a[0] / a[1] done before the next decoder overwrites them
       NSB_PH(29);
     }
@@ -1461,6 +1504,17 @@ __global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_kernel(con
 // the coarse decoder's weight gradients (stage coarse, option wgrad_all)
 __global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_coarse_tile_kernel(const __grid_constant__ KParams P) {
   render_bwd_tile_body<tl::kWgCoarse>(P);
+}
+// the deterministic-mode instantiations of the three (option "deterministic", DetParams)
+__global__ void __launch_bounds__(tl::kThreads, 2) render_bwd_tile_det_kernel(const __grid_constant__ KParams P, const __grid_constant__ DetParams D) {
+  render_bwd_tile_body<tl::kWgNone, true>(P, &D);
+}
+__global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_tile_det_kernel(const __grid_constant__ KParams P, const __grid_constant__ DetParams D) {
+  render_bwd_tile_body<tl::kWgXyz, true>(P, &D);
+}
+__global__ void __launch_bounds__(tl::kThreads, 1) render_bwd_wg_coarse_tile_det_kernel(const __grid_constant__ KParams P,
+                                                                                        const __grid_constant__ DetParams D) {
+  render_bwd_tile_body<tl::kWgCoarse, true>(P, &D);
 }
 
 }  // namespace nsb

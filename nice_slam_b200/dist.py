@@ -55,6 +55,14 @@ def reduce_sum(packed):
     return packed
 
 
+def refuse_deterministic(what):
+    """A sharded iteration over several ranks sums across them in the collective's order: library option deterministic cannot hold there."""
+    from . import _lib
+    if world()[1] > 1 and _lib.get_option("deterministic"):
+        raise RuntimeError("%s: option deterministic does not extend to %d ranks (their sums follow the collective's order); "
+                           "turn deterministic off or run on one GPU" % (what, world()[1]))
+
+
 class PeerExchange:
     """NVLink peer-memory exchange buffers for the *_peers kernels (include/nice_slam_b200.h): one symmetric buffer per rank, mapped on
     every rank through torch's symmetric-memory allocator (the plumbing); the exchanges themselves happen inside our kernels.
@@ -108,6 +116,7 @@ class ShardedTrackingIteration:
         """exchange: 'auto' = in-kernel exchanges over NVLink peer memory when available, else NCCL; 'nccl' = NCCL collectives."""
         from .renderer import require_default_sampling
         require_default_sampling(ctx.r, "ShardedTrackingIteration")
+        refuse_deterministic("ShardedTrackingIteration")
         self.ctx = ctx                      # steps.IterationContext(kind='track')
         dev = ctx.dev
         self.res = torch.empty(ctx.n, dtype=torch.float64, device=dev)
@@ -224,6 +233,7 @@ class ShardedMappingIteration:
         assert ctx.kind == "map"
         from .renderer import require_default_sampling
         require_default_sampling(ctx.r, "ShardedMappingIteration")
+        refuse_deterministic("ShardedMappingIteration")
         self.ctx = ctx
         self._p = None
 

@@ -312,9 +312,9 @@ class _RenderFn(torch.autograd.Function):
 def acts_buffer(grad_decoders, levels, n, S, device):
     """(acts [k,n,S,5,32] float32 or None, acts_levels bit mask) for the stage decoders `levels` of which `grad_decoders` want weight gradients:
     the tensor-core weight-gradient kernel serves a non-empty set of fine / colour decoders from their kept layer outputs, and with the
-    library option wgrad_all any non-empty set (the middle and coarse decoders too)."""
+    library option wgrad_all or deterministic any non-empty set (the middle and coarse decoders too)."""
     wg = [lvl for lvl in LEVELS if lvl in grad_decoders and lvl in levels]
-    if not wg or not (set(wg) <= {"fine", "color"} or _lib.get_option("wgrad_all")):
+    if not wg or not (set(wg) <= {"fine", "color"} or _lib.get_option("wgrad_all") or _lib.get_option("deterministic")):
         return None, 0
     return torch.empty(len(wg), n, S, 5, 32, dtype=torch.float32, device=device), sum(1 << LEVELS.index(lvl) for lvl in wg)
 
