@@ -1109,8 +1109,15 @@ static int weight_bytes(const int* dec, int n) {
   return wb;
 }
 
+// ---- library options (their table, read by nsb_set_option and nsb_get_option, follows det_conflict below) -------------------------
+static int g_wgrad_tc = 1;         // decoder weight gradients on the tensor cores when the forward kept the layer outputs (0: FP32-FMA pass)
 static int g_wgrad_all = 0;        // weight gradients of every decoder (middle and coarse too) on the tensor cores when the forward kept their layer outputs
 static int g_deterministic = 0;    // voxel and weight gradients summed in a fixed order (nsb_det.cu); implies wgrad_all
+static int g_fwd_f16 = 0;          // tile-kernel forward with FP16 hi|lo operands (wgmma f16, K = 16 per MMA) instead of 3xTF32; see nsb_tile.cuh mma_rows
+static int g_pdl = 0;              // iteration entry points: the backward launch as a programmatic dependent of the forward launch
+static int g_split_model = 1;      // tile kernels: per-decoder items only while they beat all-decoder items by wave efficiency (0: split whenever N*S <= kSplitMaxPts)
+static int g_small_rays = 0;       // auto dispatch: batches of up to small_rays rays on the round-1 ray-group kernels (kernel_family)
+static int g_mlp_backend = 0;      // 0 = auto (tensor-core forward), 1 = SIMT, 2 = round-1 ray-group tensor-core kernels, 3 = tile kernels
 
 // nsb_forward_outputs / nsb_backward_args .acts_levels -> K.acts_mask (0 keeps fill_common's default): the fine and colour decoders of the stage,
 // with option wgrad_all any decoder of the stage
@@ -1137,7 +1144,6 @@ static void fill_common(KParams& K, const nsb_render_inputs* in) {
   K.accumulate_rays = 0;
   K.split = 1; K.group_done = nullptr; K.fwd_parts = nullptr; K.ray_parts = nullptr; K.ray_cnt = nullptr; K.tile_parts = nullptr; K.tile_rays = 0; K.kind_major = 0;
   memset(&K.fs, 0, sizeof(K.fs)); memset(&K.tail, 0, sizeof(K.tail));
-  K.wbytes = weight_bytes(K.dec, K.n_dec);
   K.points = nullptr; K.points_raw = nullptr; K.n_points = 0;
   K.acts_mask = in->stage == NSB_STAGE_COLOR ? 1 << NSB_COLOR : 0;      // acts_levels = 0: the colour decoder (Mapper.py:339-341, fix_fine)
   memset(&K.smp, 0, sizeof(K.smp));
@@ -1154,97 +1160,53 @@ static int sm_count() {
   return g_sm_count[dev];
 }
 
-// choose rays per CTA and warps per CTA: fill all SMs once before growing CTAs (latency-bound small batches),
-// cap CTA size by the shared-memory budget (227 KB per CTA, 1 KB kept for static shared memory)
+// CTA geometry of the FP32-FMA and round-1 kernels: fill all SMs once before growing CTAs (latency-bound small batches), up to max_pts_cap
+// points per CTA (points mode: whole chunks up to kMaxPtsPerBlock points, one "ray").  With `warps`, the FP32-FMA kernels' warps per CTA for
+// the weight image K.wbytes, capped by the shared-memory budget (227 KB per CTA, 1 KB kept for static shared memory).
 constexpr size_t kSmemCap = 226u * 1024u;
 constexpr int kMaxPtsTc = 256;            // points per CTA of the tensor-core kernels (2 tiles)
-static void choose_config(int n_items, int S, int rows, bool bwd, int wbytes, int max_warps, KParams* K, int* warps, size_t* smem,
-                          int max_pts_cap = kMaxPtsPerBlock) {
+static void choose_config(KParams& K, bool bwd, int max_pts_cap, int* warps = nullptr, size_t* smem = nullptr) {
   const int sms = sm_count();
-  int r_cap = max_pts_cap / S; if (r_cap < 1) r_cap = 1; if (r_cap > kMaxRaysPerBlock) r_cap = kMaxRaysPerBlock;
-  int r = (n_items + sms - 1) / sms; if (r < 1) r = 1; if (r > r_cap) r = r_cap;
-  const int max_pts = ((r * S + kChunk - 1) / kChunk) * kChunk;
-  const int chunks = max_pts / kChunk;
-  int w = chunks < max_warps ? chunks : max_warps;
-  while (w > 1 && smem_layout(wbytes, max_pts, r, w, rows, bwd, nullptr, nullptr) > kSmemCap) w--;
+  if (K.points != nullptr) {
+    int ppb = ((K.n_points + sms - 1) / sms + kChunk - 1) / kChunk * kChunk;
+    if (ppb > kMaxPtsPerBlock) ppb = kMaxPtsPerBlock; if (ppb < kChunk) ppb = kChunk;
+    K.rays_per_block = ppb; K.max_pts = ppb; K.max_rays = 1;
+  } else {
+    int r_cap = max_pts_cap / K.S; if (r_cap < 1) r_cap = 1; if (r_cap > kMaxRaysPerBlock) r_cap = kMaxRaysPerBlock;
+    int r = (K.in.n_rays + sms - 1) / sms; if (r < 1) r = 1; if (r > r_cap) r = r_cap;
+    K.rays_per_block = r; K.max_pts = ((r * K.S + kChunk - 1) / kChunk) * kChunk; K.max_rays = r;
+  }
+  if (warps == nullptr) return;
+  const int rows = bwd ? kRowsBwd : kRowsFwd, chunks = K.max_pts / kChunk;
+  int w = chunks < 8 ? chunks : 8;
+  while (w > 1 && smem_layout(K.wbytes, K.max_pts, K.max_rays, w, rows, bwd, nullptr, nullptr) > kSmemCap) w--;
   const int rounds = (chunks + w - 1) / w;
-  w = (chunks + rounds - 1) / rounds;                    // same number of rounds with balanced warps
-  K->rays_per_block = r; K->max_pts = max_pts; K->max_rays = r;
+  if (K.points == nullptr) w = (chunks + rounds - 1) / rounds;     // same number of rounds with balanced warps
   *warps = w;
-  *smem = smem_layout(wbytes, max_pts, r, w, rows, bwd, nullptr, nullptr);
+  *smem = smem_layout(K.wbytes, K.max_pts, K.max_rays, w, rows, bwd, nullptr, nullptr);
 }
+static int cta_count(const KParams& K) { return ((K.points != nullptr ? K.n_points : K.in.n_rays) + K.rays_per_block - 1) / K.rays_per_block; }
 
-static int g_split_model = 1;      // tile kernels: per-decoder items only while they beat all-decoder items by wave efficiency (0: split whenever N*S <= kSplitMaxPts)
-static int g_pdl = 0;              // iteration entry points: the backward launch as a programmatic dependent of the forward launch
-static int g_fwd_f16 = 0;          // tile-kernel forward with FP16 hi|lo operands (wgmma f16, K = 16 per MMA) instead of 3xTF32; see nsb_tile.cuh mma_rows
-static int g_wgrad_tc = 1;         // decoder weight gradients on the tensor cores when the forward kept the layer outputs (0: FP32-FMA pass)
-static int g_mlp_backend = 0;      // 0 = auto (tensor-core forward), 1 = SIMT, 2 = round-1 ray-group tensor-core kernels, 3 = tile kernels
 static size_t tc_total_smem(int max_pts, int max_rays, bool bwd = false) {
   return ((tc::tc_smem_bytes(bwd) + 127) & ~size_t(127)) + smem_layout(0, max_pts, max_rays, 0, 0, bwd, nullptr, nullptr);
 }
 
-// ---- decoder-parallel CTAs: workspace layout and launch policy ------------------------------------------------------------------
-constexpr int kSplitMaxRays = 256;
-static size_t split_counters_bytes(int n_rays) { return align16((size_t)n_rays * sizeof(int)); }
-static size_t old_split_workspace_bytes(int n_rays, int S) {
-  if (n_rays < 1 || n_rays > kSplitMaxRays || S < 1) return 0;
-  const size_t fwd = (size_t)3 * n_rays * S * sizeof(float4), bwd = (size_t)3 * n_rays * 6 * sizeof(double);
-  return split_counters_bytes(n_rays) + (fwd > bwd ? fwd : bwd);
-}
-// ---- tile kernels: workspace = [16 B | ray completion counters (N ints) | per-item scratch] -----------------------------------------
-// per-item scratch: forward = decoder outputs [split][N*S] float4 (only when items are split per decoder; otherwise they live in fo.raw),
-// backward = ray-gradient parts [tiles * split][kMaxTileRays][6] f64.  Items are split per decoder for batches of up to kSplitMaxPts points
-// (finer granularity for small and medium batches); larger batches evaluate all decoders of a tile in one CTA.
+// ---- the split workspace: scratch of the tile kernels' items and of the round-1 kernels' decoder-parallel CTAs ---------------------
+// Tile kernels' per-item scratch: forward = decoder outputs [split][N*S] float4 (only when items are split per decoder; otherwise they live
+// in fo.raw), backward = ray-gradient parts [tiles * split][kMaxTileRays][6] f64.  Items are split per decoder for batches of up to
+// kSplitMaxPts points (finer granularity for small and medium batches); larger batches evaluate all decoders of a tile in one CTA.
 constexpr long long kSplitMaxPts = 262144;
+constexpr int kSplitMaxRays = 256;        // round-1 kernels: decoder-parallel CTAs for batches of up to this many rays
 static long long tile_count(long long n_points) { return (n_points + tc::TM - 1) / tc::TM; }
 static int tile_rays(int S) { const int r = (tc::TM - 1) / S + 2; return r < tl::kMaxTileRays ? r : tl::kMaxTileRays; }
-// Layout: [scratch ... | ray counters (N ints) at the very END of the buffer].  The counters must stay zero between launches (the completing
-// CTA resets them) while the scratch is left dirty; anchoring the counters at the end keeps the two apart when one buffer, sized for a
-// capacity, serves batches of varying size (the mapper's bbox pre-filter changes N every iteration): counters of any N <= capacity live
-// in the last 4 * capacity bytes, which no scratch of a batch <= capacity reaches (the sizing below is monotone in N).
+// per-item scratch of one tile launch
 static size_t tile_scratch_bytes(int N, int S, int split, bool bwd) {
   const long long NS = (long long)N * S;
   return bwd ? (size_t)tile_count(NS) * split * tile_rays(S) * 6 * sizeof(double) : (split > 1 ? (size_t)split * NS * sizeof(float4) : 0);
 }
-static size_t tile_ws_need(int N, int S, int split, bool bwd) { return 16 + align16((size_t)N * sizeof(int)) + align16(tile_scratch_bytes(N, S, split, bwd)); }
-// Block order of a launch of `tiles` x `split` items at ctas_per_sm resident CTAs per SM (tl::item_of_block).  When the whole launch is
-// resident at once, the block scheduler gives blocks 0 .. sms-1 one SM each; where the later blocks go does not follow that order
-// (tools/item_timing.py, H100, 225 blocks: block sms + j shares block j's SM 16 % of the time).  Such a launch takes its items decoder-major,
-// the fine decoder's first: its tiles <= sms fine items are then all in the first round, and no SM runs two of them (tile-major: the 200-ray
-// launches' last SM ran two fine items in 59 of 60 launches).  A launch of several rounds keeps tile-major order, which mixes the kinds in
-// every round (decoder-major: the 996-ray mapping backward, 748 items, ran 9 % slower).  Kernels of one CTA per SM share no SM: tile-major.
-static int item_order(long long tiles, int split, int ctas_per_sm) {
-  return ctas_per_sm > 1 && split > 1 && tiles * split <= (long long)ctas_per_sm * sm_count();
-}
-// The tile launch K in the caller's split workspace: items per tile (split), their block order, ray-completion counters, per-item scratch
-static int plan_tile_ws(KParams& K, void* ws, size_t bytes, bool bwd, int ctas_per_sm) {
-  const int N = K.in.n_rays, S = K.S, n_dec = K.n_dec;
-  bytes &= ~size_t(15);
-  int split = ((long long)N * S <= kSplitMaxPts && n_dec > 1) ? n_dec : 1;
-  if (split > 1 && g_split_model) {
-    // Splitting a tile's decoders over CTAs buys parallelism for batches that do not fill the GPU, at the price of one prologue / ray-completion
-    // pass per decoder: measured on the configs[4] sweep, a per-decoder item sustains ~0.81x (three decoders) of the throughput of the same work
-    // inside all-decoder items.  Once the tiles alone fill the resident slots (two CTAs per SM), compare the two forms by their wave efficiency.
-    const long long tiles = tile_count((long long)N * S), slots = 2ll * sm_count();
-    auto wave_eff = [&](long long items) { const long long waves = (items + slots - 1) / slots; return (double)items / (double)(waves * slots); };
-    const double eff_one = wave_eff(tiles), eff_split = wave_eff(tiles * n_dec) * (1.0 - 0.095 * (n_dec - 1));
-    if (tiles >= slots && eff_one >= eff_split) split = 1;
-  }
-  if (bytes < tile_ws_need(N, S, split, bwd)) split = 1;
-  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15) || bytes < tile_ws_need(N, S, split, bwd)) {
-    set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", N, S); return NSB_ERR_ARG; }
-  K.split = split;
-  K.kind_major = item_order(tile_count((long long)N * S), split, ctas_per_sm);
-  K.ray_cnt = reinterpret_cast<int*>(static_cast<char*>(ws) + bytes - align16((size_t)N * sizeof(int)));
-  if (bwd) { K.ray_parts = static_cast<double*>(ws); K.tile_rays = tile_rays(S); }
-  else K.tile_parts = split > 1 ? static_cast<float4*>(ws) : reinterpret_cast<float4*>(K.fo.raw);
-  return NSB_OK;
-}
-// Deterministic mode's share of the split workspace, placed right above the largest per-item scratch a batch of N rays can use (split_scratch_bytes,
-// monotone in N, like the region itself: a buffer sized for a capacity keeps it clear of the ray counters of every batch up to that
-// capacity, which sit at the END of the buffer and must stay zero between calls): per stage decoder (up to three) dL/dc [N*S][32] and
-// coordinates [N*S][3] of its points, per-tile weight-gradient images of the stage's decoders (the middle, fine and colour decoders' at most),
-// and the sort of the ordered voxel reduction (reused grid after grid).
+// Deterministic mode's buffers: per stage decoder (up to three) dL/dc [N*S][32] and coordinates [N*S][3] of its points, per-tile
+// weight-gradient images of the stage's decoders (the middle, fine and colour decoders' at most), and the sort of the ordered voxel
+// reduction (reused grid after grid).
 struct DetWs { float* dc[3]; float* xn[3]; float* wpart[3]; void* sort; size_t sort_bytes; };
 static size_t det_ws_bytes(int N, int S, DetWs* w = nullptr, char* base = nullptr) {
   const long long NP = (long long)N * S, tiles = tile_count(NP);
@@ -1261,35 +1223,85 @@ static size_t det_ws_bytes(int N, int S, DetWs* w = nullptr, char* base = nullpt
   }
   return o;
 }
-// per-item scratch of the tile kernels that nsb_split_workspace_bytes reserves at the start of the buffer (S >= NSB_MAX_SAMPLES: for any S)
-static size_t split_scratch_bytes(int n_rays, int S) {
-  auto need_exact = [&](int n, int s) {
+// The split workspace of a batch of up to N rays of S samples (S >= NSB_MAX_SAMPLES: of any S):
+//   tile kernels:             [per-item scratch | deterministic buffers (DetWs) | ... | 16 B | ray-completion counters (N ints)]
+//   round-1 ray-group kernels: [ray-group counters (N ints) | per-decoder parts [3][N*S] float4 forward, [3][N][6] f64 backward]
+// The counters must stay zero between launches (the completing CTA resets them) while the scratch is left dirty.  One buffer, sized for a
+// capacity, serves batches of varying size (the mapper's bbox pre-filter changes N every iteration), so the tile kernels' ray counters sit
+// at the very END: those of any N <= capacity live in the last 4 * capacity bytes, which nothing placed from the start for a batch <=
+// capacity reaches, as every region is the largest a batch of up to N rays can use (the deterministic buffers sit above that scratch).
+struct SplitLayout {
+  size_t counters;        // N ints, 16-byte aligned: the buffer's last bytes (tile kernels) or its first (round-1 kernels)
+  size_t scratch, det;    // tile kernels' per-item scratch at offset 0, deterministic buffers at offset `scratch` (0 without them)
+  size_t end, tile;       // 16 B and the ray counters at the end; what the tile kernels need (scratch + det + end)
+  size_t group, bytes;    // what the round-1 kernels need (0 beyond kSplitMaxRays rays); the larger of the two: nsb_split_workspace_bytes
+};
+static SplitLayout split_layout(int N, int S, bool det) {
+  auto scratch = [&](int n, int s) {
     const int split = (long long)n * s <= kSplitMaxPts ? 3 : 1;
     const size_t a = tile_scratch_bytes(n, s, split, false), b = tile_scratch_bytes(n, s, split, true);
     return align16(a > b ? a : b);
   };
-  auto need = [&](int s) {                                  // monotone in n_rays: also covers the largest batch that still splits per decoder
+  auto up_to_n = [&](int s) {                               // also covers the largest batch that still splits per decoder
     const long long n_small = kSplitMaxPts / s;
-    const size_t a = need_exact(n_rays, s), b = need_exact((int)(n_small < n_rays ? (n_small > 0 ? n_small : 1) : n_rays), s);
+    const size_t a = scratch(N, s), b = scratch((int)(n_small < N ? (n_small > 0 ? n_small : 1) : N), s);
     return a > b ? a : b;
   };
-  size_t m = need(S);
-  if (S >= NSB_MAX_SAMPLES) for (int s = tl::kMinSamples; s < NSB_MAX_SAMPLES; s++) { const size_t v = need(s); if (v > m) m = v; }   // "any S" sizing (nsb_iteration_workspace_bytes)
-  return m;
+  SplitLayout L;
+  L.counters = align16((size_t)N * sizeof(int));
+  L.scratch = up_to_n(S);
+  if (S >= NSB_MAX_SAMPLES) for (int s = tl::kMinSamples; s < NSB_MAX_SAMPLES; s++) { const size_t v = up_to_n(s); if (v > L.scratch) L.scratch = v; }
+  L.det = det ? det_ws_bytes(N, S < NSB_MAX_SAMPLES ? S : NSB_MAX_SAMPLES) : 0;
+  L.end = 16 + L.counters;
+  L.tile = L.scratch + L.det + L.end;
+  const size_t fwd = (size_t)3 * N * S * sizeof(float4), bwd = (size_t)3 * N * 6 * sizeof(double);
+  L.group = N <= kSplitMaxRays ? L.counters + (fwd > bwd ? fwd : bwd) : 0;
+  L.bytes = L.tile > L.group ? L.tile : L.group;
+  return L;
 }
 extern "C" size_t nsb_split_workspace_bytes(int n_rays, int S) {
-  if (n_rays < 1 || S < 1) return 0;
-  size_t m = split_scratch_bytes(n_rays, S);
-  m += 16 + align16((size_t)n_rays * sizeof(int));
-  if (g_deterministic) m += det_ws_bytes(n_rays, S < NSB_MAX_SAMPLES ? S : NSB_MAX_SAMPLES);
-  const size_t old = old_split_workspace_bytes(n_rays, S);
-  return m > old ? m : old;
+  return n_rays < 1 || S < 1 ? 0 : split_layout(n_rays, S, g_deterministic).bytes;
 }
-// Decide whether `nd` CTAs per ray group beat one.  Cost model = tiles a CTA walks through x decoders it evaluates x waves.
-// On success K->rays_per_block / max_pts / max_rays / split and the scratch pointers are set.
-static bool plan_split(KParams* K, int nd, void* ws, size_t ws_bytes) {
-  const int N = K->in.n_rays, S = K->S;
-  if (nd < 2 || K->points != nullptr || !ws || N > kSplitMaxRays || ws_bytes < old_split_workspace_bytes(N, S) || (reinterpret_cast<uintptr_t>(ws) & 15)) return false;
+// Block order of a launch of `tiles` x `split` items at ctas_per_sm resident CTAs per SM (tl::item_of_block).  When the whole launch is
+// resident at once, the block scheduler gives blocks 0 .. sms-1 one SM each; where the later blocks go does not follow that order
+// (tools/item_timing.py, H100, 225 blocks: block sms + j shares block j's SM 16 % of the time).  Such a launch takes its items decoder-major,
+// the fine decoder's first: its tiles <= sms fine items are then all in the first round, and no SM runs two of them (tile-major: the 200-ray
+// launches' last SM ran two fine items in 59 of 60 launches).  A launch of several rounds keeps tile-major order, which mixes the kinds in
+// every round (decoder-major: the 996-ray mapping backward, 748 items, ran 9 % slower).  Kernels of one CTA per SM share no SM: tile-major.
+static int item_order(long long tiles, int split, int ctas_per_sm) {
+  return ctas_per_sm > 1 && split > 1 && tiles * split <= (long long)ctas_per_sm * sm_count();
+}
+// The tile launch K in the caller's split workspace (laid out by W): items per tile (split), their block order, ray-completion counters,
+// per-item scratch
+static int plan_tile_ws(KParams& K, const SplitLayout& W, void* ws, size_t bytes, bool bwd, int ctas_per_sm) {
+  const int N = K.in.n_rays, S = K.S, n_dec = K.n_dec;
+  bytes &= ~size_t(15);
+  int split = ((long long)N * S <= kSplitMaxPts && n_dec > 1) ? n_dec : 1;
+  if (split > 1 && g_split_model) {
+    // Splitting a tile's decoders over CTAs buys parallelism for batches that do not fill the GPU, at the price of one prologue / ray-completion
+    // pass per decoder: measured on the configs[4] sweep, a per-decoder item sustains ~0.81x (three decoders) of the throughput of the same work
+    // inside all-decoder items.  Once the tiles alone fill the resident slots (two CTAs per SM), compare the two forms by their wave efficiency.
+    const long long tiles = tile_count((long long)N * S), slots = 2ll * sm_count();
+    auto wave_eff = [&](long long items) { const long long waves = (items + slots - 1) / slots; return (double)items / (double)(waves * slots); };
+    const double eff_one = wave_eff(tiles), eff_split = wave_eff(tiles * n_dec) * (1.0 - 0.095 * (n_dec - 1));
+    if (tiles >= slots && eff_one >= eff_split) split = 1;
+  }
+  auto need = [&](int sp) { return align16(tile_scratch_bytes(N, S, sp, bwd)) + W.end; };
+  if (bytes < need(split)) split = 1;
+  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15) || bytes < need(split)) {
+    set_error("split_workspace missing or smaller than nsb_split_workspace_bytes(%d, %d)", N, S); return NSB_ERR_ARG; }
+  K.split = split;
+  K.kind_major = item_order(tile_count((long long)N * S), split, ctas_per_sm);
+  K.ray_cnt = reinterpret_cast<int*>(static_cast<char*>(ws) + bytes - W.counters);
+  if (bwd) { K.ray_parts = static_cast<double*>(ws); K.tile_rays = tile_rays(S); }
+  else K.tile_parts = split > 1 ? static_cast<float4*>(ws) : reinterpret_cast<float4*>(K.fo.raw);
+  return NSB_OK;
+}
+// Decide whether one CTA per decoder of a ray group beats one CTA for all of them, in the caller's split workspace.  Cost model = tiles a
+// CTA walks through x decoders it evaluates x waves.  On success K->rays_per_block / max_pts / max_rays / split and the scratch pointers are set.
+static bool plan_split(KParams* K, void* ws, size_t ws_bytes) {
+  const int N = K->in.n_rays, S = K->S, nd = K->n_dec;
+  if (nd < 2 || K->points != nullptr || !ws || N > kSplitMaxRays || (reinterpret_cast<uintptr_t>(ws) & 15)) return false;
   const int sms = sm_count();
   int r_cap = kMaxPtsTc / S; if (r_cap < 1) return false; if (r_cap > kMaxRaysPerBlock) r_cap = kMaxRaysPerBlock;
   int r1 = 0;
@@ -1299,10 +1311,12 @@ static bool plan_split(KParams* K, int nd, void* ws, size_t ws_bytes) {
   const int groups0 = (N + K->rays_per_block - 1) / K->rays_per_block;
   const int cost0 = ((groups0 + sms - 1) / sms) * tiles(K->rays_per_block) * nd, cost1 = tiles(r1);
   if (cost1 >= cost0) return false;
+  const SplitLayout W = split_layout(N, S, false);
+  if (ws_bytes < W.group) return false;
   K->rays_per_block = r1; K->max_rays = r1; K->max_pts = ((r1 * S + kChunk - 1) / kChunk) * kChunk;
   K->split = nd;
   K->group_done = static_cast<int*>(ws);
-  char* rest = static_cast<char*>(ws) + split_counters_bytes(N);
+  char* rest = static_cast<char*>(ws) + W.counters;
   K->fwd_parts = reinterpret_cast<float4*>(rest);
   K->ray_parts = reinterpret_cast<double*>(rest);
   return true;
@@ -1317,7 +1331,6 @@ static size_t tile_wg_smem_bytes() { return tl::kWgBytes + ((tile_smem_bytes(tru
 // 64 rays, the tile kernels by ~20 % from 200 rays on).  The tile kernels take tl::kMinSamples <= S <= NSB_MAX_SAMPLES, the ray-group
 // kernels S <= kMaxPtsTc; other calls fall to FP32-FMA.  Points mode follows mlp_backend alone.  Forward and backward of an iteration see
 // the same (S, n_rays) and so pick the same family (the saved ReLU bits are laid out per family).
-static int g_small_rays = 0;
 enum class Family { Tile, Group, Fma };
 static Family kernel_family(int S, int n_rays, bool points) {
   const bool tile_backend = g_mlp_backend == 0 || g_mlp_backend == 3;
@@ -1367,32 +1380,60 @@ static int launch_tile_fwd(const KParams& K, long long n_points, cudaStream_t st
   else render_fwd_tile_kernel<<<grid, tl::kThreads, tile_smem_bytes(false), st>>>(K);
   return check_cuda(cudaGetLastError(), K.points ? "render_fwd_tile_kernel(points) launch" : "render_fwd_tile_kernel launch");
 }
-// Round-1 ray-group kernels: 512 threads, <= 2 tiles of 128 points per CTA, decoder-parallel CTAs when plan_split finds them faster
+// Tile backward in the split workspace plan_tile_ws laid out: item = (tile, decoder), two CTAs per SM; decoder weight gradients (wg) one CTA
+// per SM, the coarse decoder's (stage coarse) on its own instantiation.  D: deterministic mode's instantiations, whose per-tile weight-gradient
+// images are zeroed before and summed into K.d_packed after the launch.  dependent (default input-gradient launch only): a programmatic
+// dependent launch -- the forward kernel signals `launch_dependents` when it starts, so this grid's CTAs become resident as forward CTAs retire
+// and run their set-up (accumulator slot, barrier init, first weight units through TMA) under the forward's tail; `griddepcontrol.wait` in
+// front of the first read of a forward result holds them until the forward grid has completed and flushed.
+static int launch_tile_bwd(const KParams& K, bool wg, const DetParams* D, bool dependent, cudaStream_t st) {
+  const unsigned tiles = (unsigned)tile_count((long long)K.in.n_rays * K.S), grid = tiles * K.split;
+  const size_t smem = wg ? tile_wg_smem_bytes() : tile_smem_bytes(true);
+  const bool coarse = wg && K.dec[0] == NSB_COARSE;
+  if (D != nullptr) {
+    for (int q = 0; q < K.n_dec && wg; q++)
+      if (check_cuda(cudaMemsetAsync(D->wpart[K.dec[q]], 0, (size_t)tiles * packed_floats(K.dec[q]) * 4, st), "memset weight-gradient partials"))
+        return NSB_ERR_CUDA;
+    auto* kernel = coarse ? render_bwd_wg_coarse_tile_det_kernel : wg ? render_bwd_wg_tile_det_kernel : render_bwd_tile_det_kernel;
+    kernel<<<grid, tl::kThreads, smem, st>>>(K, *D);
+    int rc = check_cuda(cudaGetLastError(), "deterministic tile backward launch");
+    for (int q = 0; q < K.n_dec && wg && !rc; q++) rc = det_tile_sum(D->wpart[K.dec[q]], (int)tiles, packed_floats(K.dec[q]), K.d_packed[K.dec[q]], st);
+    return rc;
+  }
+  if (wg) {
+    auto* kernel = coarse ? render_bwd_wg_coarse_tile_kernel : render_bwd_wg_tile_kernel;
+    kernel<<<grid, tl::kThreads, smem, st>>>(K);
+    return check_cuda(cudaGetLastError(), coarse ? "render_bwd_wg_coarse_tile_kernel launch" : "render_bwd_wg_tile_kernel launch");
+  }
+  if (dependent) {
+    cudaLaunchAttribute at; at.id = cudaLaunchAttributeProgrammaticStreamSerialization; at.val.programmaticStreamSerializationAllowed = 1;
+    const cudaLaunchConfig_t cfg = {dim3(grid), dim3(tl::kThreads), smem, st, &at, 1};
+    return check_cuda(cudaLaunchKernelEx(&cfg, render_bwd_tile_kernel, K), "render_bwd_tile_kernel launch (dependent)");
+  }
+  render_bwd_tile_kernel<<<grid, tl::kThreads, smem, st>>>(K);
+  return check_cuda(cudaGetLastError(), "render_bwd_tile_kernel launch");
+}
+// Round-1 ray-group kernels: 512 threads, <= 2 tiles of 128 points per CTA (points mode: up to kMaxPtsPerBlock points), decoder-parallel
+// CTAs when plan_split finds them faster
 static int launch_group(KParams K, bool bwd, void* ws, size_t ws_bytes, cudaStream_t st) {
-  int warps; size_t smem;
-  choose_config(K.in.n_rays, K.S, bwd ? kRowsBwd : kRowsFwd, bwd, K.wbytes, 8, &K, &warps, &smem, kMaxPtsTc);
-  plan_split(&K, K.n_dec, ws, ws_bytes);
-  const int grid = ((K.in.n_rays + K.rays_per_block - 1) / K.rays_per_block) * K.split;
+  choose_config(K, bwd, kMaxPtsTc);
+  plan_split(&K, ws, ws_bytes);
+  const int grid = cta_count(K) * K.split;
   const size_t smem_tc = tc_total_smem(K.max_pts, K.max_rays, bwd);
   if (smem_tc > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem_tc); return NSB_ERR_UNSUPPORTED; }
   if (bwd) render_bwd_tc_kernel<<<grid, tc::kThreads, smem_tc, st>>>(K);
   else render_fwd_tc_kernel<<<grid, tc::kThreads, smem_tc, st>>>(K);
-  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_tc_kernel launch" : "render_fwd_tc_kernel launch");
+  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_tc_kernel launch" : K.points ? "render_fwd_tc_kernel(points) launch" : "render_fwd_tc_kernel launch");
 }
 // FP32-FMA kernels: CTA geometry and weight-image size for the decoders of K
-static int fma_config(KParams& K, bool bwd, int* warps, size_t* smem) {
-  K.wbytes = weight_bytes(K.dec, K.n_dec);
-  choose_config(K.in.n_rays, K.S, bwd ? kRowsBwd : kRowsFwd, bwd, K.wbytes, 8, &K, warps, smem);
-  if (*smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", *smem); return NSB_ERR_UNSUPPORTED; }
-  return NSB_OK;
-}
 static int launch_fma(KParams K, bool bwd, cudaStream_t st) {
   int warps; size_t smem;
-  const int rc = fma_config(K, bwd, &warps, &smem); if (rc) return rc;
-  const int grid = (K.in.n_rays + K.rays_per_block - 1) / K.rays_per_block;
-  if (bwd) render_bwd_kernel<<<grid, warps * 32, smem, st>>>(K);
-  else render_fwd_kernel<<<grid, warps * 32, smem, st>>>(K);
-  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_kernel launch" : "render_fwd_kernel launch");
+  K.wbytes = weight_bytes(K.dec, K.n_dec);
+  choose_config(K, bwd, kMaxPtsPerBlock, &warps, &smem);
+  if (smem > kSmemCap) { set_error("shared-memory budget exceeded (%zu bytes)", smem); return NSB_ERR_UNSUPPORTED; }
+  if (bwd) render_bwd_kernel<<<cta_count(K), warps * 32, smem, st>>>(K);
+  else render_fwd_kernel<<<cta_count(K), warps * 32, smem, st>>>(K);
+  return check_cuda(cudaGetLastError(), bwd ? "render_bwd_kernel launch" : K.points ? "render_fwd_kernel(points) launch" : "render_fwd_kernel launch");
 }
 
 }  // namespace nsb
@@ -1407,26 +1448,31 @@ static bool det_conflict(int det, int backend, int wgrad_tc) {
   if (!wgrad_tc) { set_error("option deterministic needs wgrad_tc = 1 (got wgrad_tc 0)"); return true; }
   return false;
 }
-extern "C" int nsb_set_option(const char* key, int value) {
-  if (key && !strcmp(key, "deterministic")) { if (det_conflict(value != 0, g_mlp_backend, g_wgrad_tc)) return NSB_ERR_ARG; g_deterministic = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "wgrad_tc")) { if (det_conflict(g_deterministic, g_mlp_backend, value != 0)) return NSB_ERR_ARG; g_wgrad_tc = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "wgrad_all")) { g_wgrad_all = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "fwd_f16")) { g_fwd_f16 = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "pdl")) { g_pdl = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "split_model")) { g_split_model = value != 0; return NSB_OK; }
-  if (key && !strcmp(key, "small_rays")) { if (value < 0) { set_error("small_rays must be >= 0"); return NSB_ERR_ARG; } g_small_rays = value; return NSB_OK; }
-  if (key && !strcmp(key, "mlp_backend")) { if (det_conflict(g_deterministic, value, g_wgrad_tc)) return NSB_ERR_ARG; if (value < 0 || value > 3) { set_error("mlp_backend must be 0 (auto = tile kernels), 1 (FP32-FMA), 2 (round-1 ray-group tensor-core kernels) or 3 (tensor-core tile kernels)"); return NSB_ERR_ARG; } g_mlp_backend = value; return NSB_OK; }
-  set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
+// The library options: name, variable, and the check a new value must pass (NULL: any value).  Flags store value != 0.
+static const struct Option { const char* name; int* var; bool flag; bool (*ok)(int value); } kOptions[] = {
+  {"wgrad_tc", &g_wgrad_tc, true, [](int v) { return !det_conflict(g_deterministic, g_mlp_backend, v != 0); }},
+  {"wgrad_all", &g_wgrad_all, true, nullptr}, {"fwd_f16", &g_fwd_f16, true, nullptr}, {"pdl", &g_pdl, true, nullptr},
+  {"split_model", &g_split_model, true, nullptr},
+  {"small_rays", &g_small_rays, false, [](int v) { if (v < 0) set_error("small_rays must be >= 0"); return v >= 0; }},
+  {"mlp_backend", &g_mlp_backend, false, [](int v) {
+     if (det_conflict(g_deterministic, v, g_wgrad_tc)) return false;
+     if (v < 0 || v > 3) set_error("mlp_backend must be 0 (auto = tile kernels), 1 (FP32-FMA), 2 (round-1 ray-group tensor-core kernels) or 3 (tensor-core tile kernels)");
+     return v >= 0 && v <= 3; }},
+  {"deterministic", &g_deterministic, true, [](int v) { return !det_conflict(v != 0, g_mlp_backend, g_wgrad_tc); }},
+};
+static const Option* find_option(const char* key) {
+  for (const auto& o : kOptions) if (key && !strcmp(key, o.name)) return &o;
+  set_error("unknown option %s", key ? key : "(null)"); return nullptr;
 }
-
+extern "C" int nsb_set_option(const char* key, int value) {
+  const Option* o = find_option(key);
+  if (!o || (o->ok && !o->ok(value))) return NSB_ERR_ARG;
+  *o->var = o->flag ? value != 0 : value; return NSB_OK;
+}
 extern "C" int nsb_get_option(const char* key, int* value) {
   if (!value) { set_error("nsb_get_option: value is NULL"); return NSB_ERR_ARG; }
-  const struct { const char* name; int v; } opts[] = {{"wgrad_tc", g_wgrad_tc}, {"wgrad_all", g_wgrad_all}, {"fwd_f16", g_fwd_f16}, {"pdl", g_pdl},
-                                                      {"split_model", g_split_model}, {"small_rays", g_small_rays}, {"mlp_backend", g_mlp_backend},
-                                                      {"deterministic", g_deterministic}};
-  for (const auto& o : opts)
-    if (key && !strcmp(key, o.name)) { *value = o.v; return NSB_OK; }
-  set_error("unknown option %s", key ? key : "(null)"); return NSB_ERR_ARG;
+  const Option* o = find_option(key); if (!o) return NSB_ERR_ARG;
+  *value = *o->var; return NSB_OK;
 }
 
 // nsb_sampling -> K.smp; a given sample list sets the samples per ray
@@ -1466,7 +1512,7 @@ int nsb::render_forward_fused(const nsb_render_inputs* in, const nsb_forward_out
     set_error("in-kernel exchanges of a sharded forward need a tensor-core back-end and <= %d rays per rank", NSB_INLINE_MAX_RAYS); return NSB_ERR_UNSUPPORTED; }
   if (fam == Family::Tile) {
     if (!out->z_vals || !out->raw) { set_error("the tensor-core forward needs z_vals and raw outputs"); return NSB_ERR_ARG; }
-    if ((rc = plan_tile_ws(K, out->split_workspace, out->split_workspace_bytes, false, 2))) return rc;
+    if ((rc = plan_tile_ws(K, split_layout(in->n_rays, K.S, false), out->split_workspace, out->split_workspace_bytes, false, 2))) return rc;
     return launch_tile_fwd(K, (long long)in->n_rays * K.S, (cudaStream_t)stream);
   }
   if (fam == Family::Group) return launch_group(K, false, out->split_workspace, out->split_workspace_bytes, (cudaStream_t)stream);
@@ -1495,31 +1541,19 @@ extern "C" int nsb_eval_points(const nsb_render_inputs* in, const double* points
   KParams K; fill_common(K, in); memset(&K.fo, 0, sizeof(K.fo)); memset(&K.bw, 0, sizeof(K.bw));
   K.points = points; K.points_raw = raw; K.n_points = n_points; K.S = 1; K.has_gt = 0;
   if ((rc = set_attrs())) return rc;
-  // points mode: "rays_per_block" = points per CTA
-  const int sms = sm_count();
-  int ppb = (n_points + sms - 1) / sms; ppb = ((ppb + kChunk - 1) / kChunk) * kChunk;
-  if (ppb > kMaxPtsPerBlock) ppb = kMaxPtsPerBlock;
-  if (ppb < kChunk) ppb = kChunk;
-  int warps = ppb / kChunk < 8 ? ppb / kChunk : 8;
-  while (warps > 1 && smem_layout(K.wbytes, ppb, 1, warps, kRowsFwd, false, nullptr, nullptr) > kSmemCap) warps--;
-  const size_t smem = smem_layout(K.wbytes, ppb, 1, warps, kRowsFwd, false, nullptr, nullptr);
-  K.rays_per_block = ppb; K.max_pts = ppb; K.max_rays = 1;
-  const int grid = (n_points + ppb - 1) / ppb;
   const Family fam = kernel_family(K.S, 0, true);
   if (fam == Family::Tile) return launch_tile_fwd(K, n_points, (cudaStream_t)stream);
-  if (fam == Family::Group) {
-    render_fwd_tc_kernel<<<grid, tc::kThreads, tc_total_smem(K.max_pts, K.max_rays), (cudaStream_t)stream>>>(K);
-    return check_cuda(cudaGetLastError(), "render_fwd_tc_kernel(points) launch");
-  }
-  render_fwd_kernel<<<grid, warps * 32, smem, (cudaStream_t)stream>>>(K);
-  return check_cuda(cudaGetLastError(), "render_fwd_kernel(points) launch");
+  if (fam == Family::Group) return launch_group(K, false, nullptr, 0, (cudaStream_t)stream);
+  return launch_fma(K, false, (cudaStream_t)stream);
 }
 
 namespace nsb { int launch_unpack_grads(float* const d_packed[4], float* const d_flat[4], cudaStream_t st); }
 
-extern "C" size_t nsb_backward_workspace_bytes(void) {
-  size_t t = 0; for (int l = 0; l < 4; l++) t += align16((size_t)packed_floats(l) * 4); return t;
+// backward workspace: the packed weight-gradient images of the four decoders in level order; that of level l starts here
+static size_t backward_ws_offset(int l) {
+  size_t o = 0; for (int m = 0; m < l; m++) o += align16((size_t)packed_floats(m) * 4); return o;
 }
+extern "C" size_t nsb_backward_workspace_bytes(void) { return backward_ws_offset(4); }
 
 // loss.backward() at src/Tracker.py:125 / src/Mapper.py:503 (nsb_render_backward: after the default sampler)
 extern "C" int nsb_render_backward(const nsb_render_inputs* in, const nsb_backward_args* bw, void* stream) {
@@ -1559,8 +1593,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
     const int l = K.dec[i];
     if (bw->d_flat[l] != nullptr) {
       if (!bw->workspace) { set_error("d_flat requested but workspace is NULL (nsb_backward_workspace_bytes)"); return NSB_ERR_ARG; }
-      size_t off = 0; for (int m = 0; m < l; m++) off += align16((size_t)packed_floats(m) * 4);
-      K.d_packed[l] = reinterpret_cast<float*>(reinterpret_cast<char*>(bw->workspace) + off);
+      K.d_packed[l] = reinterpret_cast<float*>(reinterpret_cast<char*>(bw->workspace) + backward_ws_offset(l));
       if (check_cuda(cudaMemsetAsync(K.d_packed[l], 0, (size_t)packed_floats(l) * 4, st), "memset d_packed")) return NSB_ERR_CUDA;
       any_w = true;
     }
@@ -1568,9 +1601,6 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   // grids/weights that are not part of this stage get no gradient
   for (int l = 0; l < 4; l++) { bool used = false; for (int i = 0; i < K.n_dec; i++) used |= K.dec[i] == l; if (!used) { K.bw.d_grid[l] = nullptr; } }
   if ((rc = set_attrs())) return rc;
-  // Every launch below starts from K, so each carries the FP32-FMA geometry of the whole stage (only the FP32-FMA kernels read it).
-  int warps; size_t smem;
-  if ((rc = fma_config(K, true, &warps, &smem))) return rc;
   // Plan: with the saved ReLU masks a tensor-core launch for the decoders that only need input gradients (rays, voxels), then one for those
   // whose WEIGHT gradients are requested (the colour decoder in the mapper's colour stage, Mapper.py:339-341; with fix_fine = False also the
   // fine decoder; every decoder of the stage when the caller leaves them all trainable, as the tracker and mapper do): on the tensor cores when
@@ -1608,6 +1638,7 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   bool det_grads = any_w;
   for (int l = 0; l < 4; l++) det_grads |= K.bw.d_grid[l] != nullptr;
   const bool det = g_deterministic && det_grads;
+  const SplitLayout W = split_layout(in->n_rays, K.S, det);
   DetWs dw; memset(&dw, 0, sizeof(dw));
   if (det) {
     if (sharded) { set_error("option deterministic: the sharded backward tail sums over ranks in arrival order (turn deterministic off)"); return NSB_ERR_UNSUPPORTED; }
@@ -1617,15 +1648,12 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
                   "layer outputs (acts / acts_levels)");
         return NSB_ERR_UNSUPPORTED;
       }
-    const size_t room = bw->split_workspace_bytes & ~size_t(15);
-    const size_t base = split_scratch_bytes(in->n_rays, K.S);
-    const size_t need = base + det_ws_bytes(in->n_rays, K.S) + 16 + align16((size_t)in->n_rays * sizeof(int));
-    if (!bw->split_workspace || (reinterpret_cast<uintptr_t>(bw->split_workspace) & 15) || room < need) {
+    if (!bw->split_workspace || (reinterpret_cast<uintptr_t>(bw->split_workspace) & 15) || (bw->split_workspace_bytes & ~size_t(15)) < W.tile) {
       set_error("split_workspace smaller than nsb_split_workspace_bytes(%d, %d) with option deterministic on (size it after setting the option)",
                 in->n_rays, K.S);
       return NSB_ERR_ARG;
     }
-    det_ws_bytes(in->n_rays, K.S, &dw, static_cast<char*>(bw->split_workspace) + base);
+    det_ws_bytes(in->n_rays, K.S, &dw, static_cast<char*>(bw->split_workspace) + W.scratch);
   }
   auto det_params = [&](const KParams& P, bool wg) {
     DetParams D; memset(&D, 0, sizeof(D));
@@ -1640,47 +1668,12 @@ int nsb::render_backward_tail(const nsb_render_inputs* in, const nsb_backward_ar
   };
   for (int i = 0; i < n; i++) {
     KParams& P = L[i];
-    const unsigned tiles = (unsigned)tile_count((long long)in->n_rays * P.S);
-    if (det && (kind[i] == TileIg || kind[i] == WgTile)) {
-      if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true, kind[i] == WgTile ? 1 : 2))) return rc;
-      const DetParams D = det_params(P, kind[i] == WgTile);
-      if (kind[i] == WgTile) {
-        for (int q = 0; q < P.n_dec; q++)
-          if (check_cuda(cudaMemsetAsync(D.wpart[P.dec[q]], 0, (size_t)tiles * packed_floats(P.dec[q]) * 4, st), "memset weight-gradient partials"))
-            return NSB_ERR_CUDA;
-        if (P.dec[0] == NSB_COARSE) render_bwd_wg_coarse_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P, D);
-        else render_bwd_wg_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P, D);
-      } else {
-        render_bwd_tile_det_kernel<<<tiles * P.split, tl::kThreads, tile_smem_bytes(true), st>>>(P, D);
-      }
-      if ((rc = check_cuda(cudaGetLastError(), "deterministic tile backward launch"))) return rc;
-      for (int q = 0; q < P.n_dec && kind[i] == WgTile; q++)
-        if ((rc = det_tile_sum(D.wpart[P.dec[q]], (int)tiles, packed_floats(P.dec[q]), K.d_packed[P.dec[q]], st))) return rc;
-      continue;
-    }
+    const bool wg = kind[i] == WgTile;
     if (kind[i] == GroupIg) rc = launch_group(P, true, bw->split_workspace, bw->split_workspace_bytes, st);
     else if (kind[i] == Fma) rc = launch_fma(P, true, st);
-    else if ((rc = plan_tile_ws(P, bw->split_workspace, bw->split_workspace_bytes, true, kind[i] == WgTile ? 1 : 2))) return rc;
-    else if (kind[i] == WgTile && P.dec[0] == NSB_COARSE) {         // (stage coarse: the coarse decoder alone)
-      render_bwd_wg_coarse_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
-      rc = check_cuda(cudaGetLastError(), "render_bwd_wg_coarse_tile_kernel launch");
-    } else if (kind[i] == WgTile) {
-      render_bwd_wg_tile_kernel<<<tiles * P.split, tl::kThreads, tile_wg_smem_bytes(), st>>>(P);
-      rc = check_cuda(cudaGetLastError(), "render_bwd_wg_tile_kernel launch");
-    } else if (after_forward && !any_w && g_pdl) {
-      // Programmatic dependent launch: the forward kernel signals `launch_dependents` when it starts, so this grid's CTAs become resident as
-      // forward CTAs retire and run their set-up (accumulator slot, barrier init, first weight units through TMA) under the forward's tail
-      // (ray compositing, the last CTA's loss seeds / peer exchange); `griddepcontrol.wait` in front of the first read of a forward
-      // result holds them until the forward grid has completed and flushed.
-      cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-      cfg.gridDim = dim3(tiles * P.split); cfg.blockDim = dim3(tl::kThreads); cfg.dynamicSmemBytes = tile_smem_bytes(true); cfg.stream = st;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      rc = check_cuda(cudaLaunchKernelEx(&cfg, render_bwd_tile_kernel, P), "render_bwd_tile_kernel launch (dependent)");
-    } else {
-      render_bwd_tile_kernel<<<tiles * P.split, tl::kThreads, tile_smem_bytes(true), st>>>(P);
-      rc = check_cuda(cudaGetLastError(), "render_bwd_tile_kernel launch");
+    else if (!(rc = plan_tile_ws(P, W, bw->split_workspace, bw->split_workspace_bytes, true, wg ? 1 : 2))) {
+      const DetParams D = det_params(P, wg);
+      rc = launch_tile_bwd(P, wg, det ? &D : nullptr, after_forward && !any_w && g_pdl, st);
     }
     if (rc) return rc;
   }
