@@ -842,8 +842,10 @@ __device__ __forceinline__ void issue_bwd_layer(Issuer& I, const TileSmem& t, in
 // the xyz one took that kernel past 255 registers (spills).
 enum { kWgNone = 0, kWgXyz = 1, kWgCoarse = 2 };
 __device__ __forceinline__ int bwd_dpe_off(int r) { return (r >> 6) * (64 * 32) + (r & 63) * 4; }
-// kDet (deterministic mode): the per-warp bias partials are added in warp order through shared memory and stored, not reduced by atomics
-// (w->dpk is then this tile's own zeroed partial image, which every other element of receives exactly one reduction per tile).
+// Bias gradients: the per-warp column sums are added in warp order through shared memory, so a tile contributes one sum per element.  The
+// default kernels add that sum to w->dpk with one atomic (the order of the atomics is then the order of the tiles alone, not of the tiles'
+// eight warps); kDet (deterministic mode) stores it, w->dpk being this tile's own zeroed partial image, which every other element of receives
+// exactly one reduction per tile.
 __device__ __forceinline__ float* det_bias_smem() { __shared__ float s[8 * 64]; return s; }
 template <int WG, bool kDet = false>
 __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t, Issuer& I, const BwdExtra& X, int lv, const PointGeom& G, int hb, uint32_t hdr_parity,
@@ -915,20 +917,16 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
     if (cg == 0) {
       const float sb = warp_colsum16(go, lane);
       const int col = colsum_col(lane);
-      if ((lane & 1) == 0 && col < DW.no) {
-        if constexpr (kDet) det_bias_smem()[warp * 64 + col] = sb;
-        else atomicAdd(w->dpk + DW.o_bo + col, sb);
-      }
+      if ((lane & 1) == 0 && col < DW.no) det_bias_smem()[warp * 64 + col] = sb;
     }
-    if constexpr (kDet) {
-      __syncthreads();
-      if ((int)threadIdx.x < DW.no) {
-        float s = 0.0f;
-        for (int wp = 0; wp < 4; wp++) s = __fadd_rn(s, det_bias_smem()[wp * 64 + threadIdx.x]);
-        w->dpk[DW.o_bo + threadIdx.x] = s;
-      }
-      __syncthreads();
+    __syncthreads();
+    if ((int)threadIdx.x < DW.no) {
+      float s = 0.0f;
+      for (int wp = 0; wp < 4; wp++) s = __fadd_rn(s, det_bias_smem()[wp * 64 + threadIdx.x]);
+      if constexpr (kDet) w->dpk[DW.o_bo + threadIdx.x] = s;
+      else atomicAdd(w->dpk + DW.o_bo + threadIdx.x, s);
     }
+    __syncthreads();
   }
 #pragma unroll 1
   for (int i = 4; i >= 0; i--) {
@@ -954,22 +952,19 @@ __device__ __forceinline__ void epi_backward(const KParams& P, const TileSmem& t
       float sc = 0.0f;
       if constexpr (WG != kWgCoarse) sc = frag_colsum(d1, lane);
       const int col = frag_colsum_col(lane);
-      if constexpr (kDet) {
-        float* sbias = det_bias_smem();
-        sbias[warp * 64 + col] = sb;
-        if constexpr (WG != kWgCoarse) sbias[warp * 64 + 32 + col] = sc;
-        __syncthreads();
-        if ((int)threadIdx.x < (WG != kWgCoarse ? 64 : 32)) {
-          const int c = threadIdx.x & 31;
-          float s = 0.0f;
-          for (int wp = 0; wp < kThreads / 32; wp++) s = __fadd_rn(s, sbias[wp * 64 + threadIdx.x]);
-          w->dpk[(threadIdx.x < 32 ? DW.o_b : DW.o_bc) + 32 * i + c] = s;
-        }
-        __syncthreads();
-      } else {
-        atomicAdd(w->dpk + DW.o_b + 32 * i + col, sb);
-        if constexpr (WG != kWgCoarse) atomicAdd(w->dpk + DW.o_bc + 32 * i + col, sc);
+      float* sbias = det_bias_smem();
+      sbias[warp * 64 + col] = sb;
+      if constexpr (WG != kWgCoarse) sbias[warp * 64 + 32 + col] = sc;
+      __syncthreads();
+      if ((int)threadIdx.x < (WG != kWgCoarse ? 64 : 32)) {
+        const int c = threadIdx.x & 31;
+        float s = 0.0f;
+        for (int wp = 0; wp < kThreads / 32; wp++) s = __fadd_rn(s, sbias[wp * 64 + threadIdx.x]);
+        float* const dst = w->dpk + (threadIdx.x < 32 ? DW.o_b : DW.o_bc) + 32 * i + c;
+        if constexpr (kDet) *dst = s;
+        else atomicAdd(dst, s);
       }
+      __syncthreads();
     }
     fence_proxy_async();
     wg_bar_sync();                                               // this warpgroup's rows of G / DU are written -> its MMAs

@@ -8,6 +8,10 @@
   * the deterministic gradients stay within float32 summation-order noise of the default mode's;
   * a backward whose split workspace was sized with the option off is refused, not run (drop-in and fused iteration);
   * one fused IterationContext serves a smaller then a larger batch and matches a fresh context bit for bit;
+  * exact invariants (torch.equal, on non-zero tensors, with the kernels that ran checked in a profiler trace): the mode leaves the forward
+    and the ray gradients unchanged; channels-last and NCDHW grids give the same bits; compact (val[mask]) voxel gradients equal the dense
+    ones at the mask, drop-in and fused; a split workspace left full of NaN by an earlier call gives the same bits as a zeroed one;
+  * the mode's dispatch edges: S < 8 (ray-group kernels) refused by name, small_rays ignored, a tracking call on the default kernels;
   * two replays of the golden sequences (FusedSLAM, coarse mapper off and on) give equal poses, losses, grids, decoders and checkpoint
     contents, within test_gpu_slam's bars against the reference."""
 import os
@@ -18,7 +22,10 @@ import torch
 
 import scene_util as su
 from gpu_util import make_renderer, rel
+from oracle import f64_ref as fr
 from oracle import torch_port as tp
+from test_gpu_f64 import GRIDS
+from test_gpu_wgrad_all import kernel_names
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -38,9 +45,8 @@ class option:
 
     def __exit__(self, *exc):
         from nice_slam_b200 import _lib
-        for k in ("deterministic", "split_model", "wgrad_all", "mlp_backend", "wgrad_tc"):
-            if k in self.prev:
-                _lib.set_option(k, self.prev[k])
+        for k in sorted(self.prev, key=lambda k: k != "deterministic"):      # (deterministic first: it refuses some values of the others)
+            _lib.set_option(k, self.prev[k])
 
 
 # ------------------------------------------------------------------------------------ the ordered reduction alone
@@ -298,6 +304,305 @@ def test_iteration_workspace_sized_with_the_option_off_names_it():
         with pytest.raises(RuntimeError, match="deterministic"):
             ctx.run(c, dec, ro, rd, gd, gc.float().contiguous())
     torch.cuda.synchronize()
+
+
+# ------------------------------------------------------------------------------------ exact invariants
+FWD = ("depth", "var", "rgb", "raw", "z_vals", "masks", "d_rays_o", "d_rays_d")     # the same arithmetic in every mode and layout
+FORMS = {"grids": lambda stage: (), "color_wg": lambda stage: ("color",), "all": lambda stage: fr.STAGE_DECODERS[stage]}
+
+
+def render_call(stage, n_rays=97, form="grids", n_samples=17, n_surface=16, seed=3000, channels_last=True, voxel_masks=None, attempts=3):
+    """One drop-in render_batch_ray (soft room0 scene, the grids of the stage graded, the decoders of `form` trainable) and the backward of
+    seeded random cotangents of depth, var and rgb, traced.  voxel_masks {grid key: [D, H, W] bool}: that grid takes the reference mapper's
+    val[mask] parameterisation (Mapper.py:317-333, the mask repeated over the channels), which the renderer serves with compact gradients.
+    -> (dict of outputs and gradients, kernel names of the call).  A trace without a render forward and a render backward kernel has lost
+    device records (see test_gpu_wgrad_all._profiled), and the call is run again."""
+    from torch.profiler import ProfilerActivity, profile
+    from nice_slam_b200.masked import MaskedVoxels
+    sc, grids, dec_state = _scene()
+    gdec = FORMS[form](stage)
+    for _ in range(attempts):
+        renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, channels_last=channels_last, n_samples=n_samples, n_surface=n_surface)
+        ro, rd, gd, _ = su.make_rays(sc, n_rays, seed=seed)
+        g = torch.Generator().manual_seed(seed)
+        cot = (torch.randn(n_rays, dtype=torch.float64, generator=g), torch.randn(n_rays, dtype=torch.float64, generator=g),
+               torch.randn(n_rays, 3, generator=g))
+        cot = tuple(x.to(DEV) for x in cot)
+        r1, r2 = ro.to(DEV).requires_grad_(True), rd.to(DEV).requires_grad_(True)
+        for n, p in dec.named_parameters():
+            p.requires_grad_(n.split("_decoder.")[0] in gdec)
+        leaves = {}
+        for k in list(c):
+            c[k] = c[k].detach()
+            if k not in GRIDS[stage]:
+                continue
+            if voxel_masks is not None and k in voxel_masks:
+                m5 = voxel_masks[k].to(DEV).unsqueeze(0).unsqueeze(0).expand_as(c[k])
+                val = c[k][m5].clone().requires_grad_(True)
+                full = c[k].clone()
+                full[m5] = val
+                leaves[k], c[k] = val, full
+            else:
+                c[k] = c[k].clone().requires_grad_(True)
+                leaves[k] = c[k]
+        aux = {}
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            d, u, col = renderer.render_batch_ray(c, dec, r2, r1, DEV, stage, gt_depth=gd.to(DEV), aux=aux)
+            ((d * cot[0]).sum() + (u * cot[1]).sum() + (col * cot[2]).sum()).backward()
+            torch.cuda.synchronize()
+        names = kernel_names(prof)
+        if any(x.startswith("render_fwd") for x in names) and any(x.startswith("render_bwd") for x in names):
+            break
+    if voxel_masks is not None:                                   # the compact path served the masked grids
+        assert sum(isinstance(v, MaskedVoxels) for v in renderer._mask_cache.values()) == len(voxel_masks), renderer._mask_cache
+    # (the saved ReLU words of the stage's decoders: word 5 * dec_pos + layer; the others are not written.  rgb: the colour stage's alone)
+    out = dict(depth=d.detach(), var=u.detach(), raw=aux["raw"], z_vals=aux["z_vals"],
+               masks=aux["masks"][..., : 5 * len(fr.STAGE_DECODERS[stage])], d_rays_o=r1.grad, d_rays_d=r2.grad)
+    if stage == "color":
+        out["rgb"] = col.detach()
+    out.update({"d_" + k: v.grad for k, v in leaves.items()})
+    out.update({"d_" + n: p.grad for n, p in dec.named_parameters() if p.grad is not None})
+    assert set(k.split("_decoder.")[0][2:] for k in out if "_decoder." in k) == set(gdec), sorted(out)
+    return out, names
+
+
+def backward_kernel(stage, form, det):
+    """The tile backward kernel that produces the call's voxel (and, with decoders graded, weight) gradients."""
+    base = "render_bwd_tile" if form == "grids" else "render_bwd_wg_coarse_tile" if stage == "coarse" else "render_bwd_wg_tile"
+    return base + ("_det" if det else "") + "_kernel"
+
+
+def check_kernels(names, stage, form, det):
+    """The intended backward ran, and every render backward of the call is of the mode's family (kDet or default)."""
+    bwd = sorted(set(x for x in names if x.startswith("render_bwd")))
+    assert backward_kernel(stage, form, det) in bwd, (stage, form, det, bwd)
+    assert all(("_det_" in x) == bool(det) for x in bwd), (det, bwd)
+    assert not any(x.startswith("render_fwd_tc") or x == "render_bwd_kernel" for x in names), names
+
+
+def assert_bits(a, b, keys, what):
+    """torch.equal on each of `keys` (every decoder gradient for keys = None), each non-zero; decoder gradients non-zero per decoder."""
+    keys = sorted(a) if keys is None else [k for k in keys if k != "rgb" or "rgb" in a or "rgb" in b]
+    assert set(keys) <= set(a) and set(keys) <= set(b), (what, sorted(a), sorted(b))
+    differ = [k for k in keys if not torch.equal(a[k], b[k])]
+    assert not differ, (what, [(k, float((a[k].double() - b[k].double()).abs().max())) for k in differ])
+    for k in keys:
+        if "_decoder." not in k:
+            assert float(a[k].double().abs().max()) > 0, (what, k)
+    for lvl in set(k.split("_decoder.")[0] for k in keys if "_decoder." in k):
+        assert max(float(a[k].abs().max()) for k in keys if k.startswith(lvl + "_decoder.")) > 0, (what, lvl)
+
+
+@pytest.mark.parametrize("stage,form", [(s, "grids") for s in ("coarse", "middle", "fine", "color")] + [("color", "color_wg")] +
+                         [(s, "all") for s in ("coarse", "middle", "fine", "color")])
+def test_mode_leaves_forward_and_ray_gradients_unchanged(stage, form):
+    """The forward is the same kernel in both modes, and the kDet backward differs from the default one only in where dL/dc and the weight
+    partials go: the ray parts are summed in (tile, decoder) order either way.  Form "all" is set beside option wgrad_all, which puts every
+    decoder's weight gradients on the same kernel family as the mode does."""
+    with option(deterministic=0, wgrad_all=int(form == "all")):
+        dflt, nd = render_call(stage, form=form)
+    with option(deterministic=1):
+        det, nt = render_call(stage, form=form)
+    check_kernels(nd, stage, form, 0)
+    check_kernels(nt, stage, form, 1)
+    assert_bits(det, dflt, FWD, "mode %s %s" % (stage, form))
+
+
+@pytest.mark.parametrize("det", [1, 0])
+@pytest.mark.parametrize("stage,form", [("coarse", "all"), ("middle", "grids"), ("fine", "all"), ("color", "color_wg"), ("color", "all")])
+def test_channels_last_and_ncdhw_grids_give_identical_bits(stage, form, det):
+    """gather_issue loads the same floats through either layout's addressing and gather_consume / gather_tile_kt run one fmaf chain on them,
+    so the forward and the ray gradients are bit-identical; in deterministic mode the ordered voxel sum keys a voxel by its index, not its
+    address, so every voxel and decoder gradient is too."""
+    runs = {}
+    for cl in (True, False):
+        with option(deterministic=det, wgrad_all=1):
+            runs[cl], names = render_call(stage, form=form, channels_last=cl, seed=3100)
+        check_kernels(names, stage, form, det)
+    assert_bits(runs[False], runs[True], None if det else FWD, "layout %s %s det=%d" % (stage, form, det))
+
+
+def _voxel_masks(stage, kind):
+    """{grid key: [D, H, W] bool} for the grids of the stage: 'random' selects about 70 % of the voxels; 'half' leaves out the voxels of
+    x index < W / 2, so every corner of the samples in that half takes the slot -1 path."""
+    sc, grids, _ = _scene()
+    g = torch.Generator().manual_seed(31)
+    out = {}
+    for k in GRIDS[stage]:
+        D, H, W = grids[k].shape[2:]
+        if kind == "random":
+            out[k] = torch.rand(D, H, W, generator=g) < 0.7
+        else:
+            out[k] = torch.ones(D, H, W, dtype=torch.bool)
+            out[k][:, :, : W // 2] = False
+    return out
+
+
+@pytest.mark.parametrize("kind", ["random", "half"])
+@pytest.mark.parametrize("stage", ["coarse", "middle", "fine", "color"])
+def test_compact_voxel_gradients_equal_the_dense_ones(stage, kind):
+    """The ordered voxel sum takes each voxel's (point, corner) list in the same order whether its key is a slot or a linear voxel index:
+    the drop-in val[mask] gradient equals the dense call's gradient at the mask, bit for bit, with every decoder graded."""
+    masks = _voxel_masks(stage, kind)
+    with option(deterministic=1):
+        dense, nd = render_call(stage, form="all", seed=3200)
+        comp, nc = render_call(stage, form="all", seed=3200, voxel_masks=masks)
+    check_kernels(nd, stage, "all", 1)
+    check_kernels(nc, stage, "all", 1)
+    assert_bits(comp, dense, FWD + tuple(k for k in dense if "_decoder." in k), "compact %s %s" % (stage, kind))
+    for k, m in masks.items():
+        g = dense["d_" + k]
+        m5 = m.to(DEV).unsqueeze(0).unsqueeze(0).expand_as(g)
+        want = g[m5]
+        assert float(want.abs().max()) > 0, k
+        assert float(g[~m5].abs().max()) > 0, k                   # samples did reach the voxels left out
+        assert torch.equal(comp["d_" + k], want), (k, float((comp["d_" + k] - want).abs().max()))
+
+
+@pytest.mark.parametrize("stage", ["color", "coarse"])
+def test_masked_iteration_compact_gradients_equal_the_dense_ones(stage):
+    """The fused mapping iteration (IterationContext) with MaskedVoxels: its compact gradients equal the dense context's at the mask bit for
+    bit (test_gpu_parity.test_masked_mapping_iteration_packed_block holds the default mode to rel < 1e-5)."""
+    from nice_slam_b200.masked import MaskedVoxels
+    from nice_slam_b200.steps import IterationContext
+    sc, grids, dec_state = _scene()
+    masks = _voxel_masks(stage, "random")
+    keys = tuple(masks)
+    decs = ("coarse",) if stage == "coarse" else ("middle", "fine", "color")
+    with option(deterministic=1):
+        renderer, c, dec = make_renderer(sc, grids, dec_state, DEV)
+        ro, rd, gd, gc = (t.to(DEV).contiguous() for t in su.make_rays(sc, 330, seed=3300))
+        gc = gc.float().contiguous()
+        kw = dict(kind="map", grad_grids=keys, grad_decoders=decs, coarse_mapper=stage == "coarse")
+        dense = IterationContext(renderer, 330, stage, DEV, **kw)
+        dense.run(c, dec, ro, rd, gd, gc)
+        mv = {k: MaskedVoxels(c[k], masks[k]) for k in keys}
+        ctx = IterationContext(renderer, 330, stage, DEV, masked=mv, **kw)
+        ctx.run(c, dec, ro, rd, gd, gc)
+        torch.cuda.synchronize()
+    assert torch.equal(ctx.loss, dense.loss)
+    for k in keys:
+        m5 = masks[k].to(DEV).unsqueeze(0).unsqueeze(0).expand_as(dense.d_grid[k])
+        want = dense.d_grid[k][m5]
+        assert float(want.abs().max()) > 0, k
+        assert torch.equal(mv[k].to_reference(ctx.d_grid[k]), want), (k, float((mv[k].to_reference(ctx.d_grid[k]) - want).abs().max()))
+    for lvl in decs:
+        assert float(dense.d_flat[lvl].abs().max()) > 0 and torch.equal(ctx.d_flat[lvl], dense.d_flat[lvl]), lvl
+
+
+def _poison_split_workspace(monkeypatch):
+    """Every drop-in forward's split workspace comes back from _forward_setup filled with 0xFF bytes (NaN as float32) -- as a workspace
+    reused by an earlier call may be -- except the ray-completion counters at its end and the 16 bytes in front of them, which split_layout
+    (nsb_render.cu) requires to start at zero.  Any NaN in a result is then a read of a region the call did not write first."""
+    import nice_slam_b200.renderer as R
+    setup = R._forward_setup
+
+    def poisoned(call, ro):
+        res = setup(call, ro)
+        split = res[3][5]
+        if split is not None:
+            keep = 16 + (4 * ro.shape[0] + 15) // 16 * 16
+            assert split.numel() > keep
+            split[: split.numel() - keep].fill_(0xFF)
+        return res
+
+    monkeypatch.setattr(R, "_forward_setup", poisoned)
+
+
+POISON_CASES = [("coarse", 97, 33, "all", False), ("coarse", 1408, 256, "grids", True), ("fine", 97, 256, "grids", False),
+                ("fine", 1408, 33, "all", True), ("color", 97, 33, "color_wg", True), ("color", 1408, 33, "grids", False),
+                ("color", 97, 256, "all", False), ("color", 1408, 256, "color_wg", False)]
+
+
+@pytest.mark.parametrize("det", [1, 0])
+@pytest.mark.parametrize("stage,n_rays,S,form,compact", POISON_CASES)
+def test_dirty_split_workspace_gives_the_bits_of_a_clean_one(stage, n_rays, S, form, compact, det, monkeypatch):
+    """The same call on a zeroed and on a NaN-filled split workspace (tile kernels: S >= 8, small_rays 0).  Deterministic mode: every output
+    and gradient bit-identical.  Default mode: forward and ray gradients bit-identical, voxel and weight gradients (float atomics) finite and
+    within float32 summation-order noise."""
+    ns, nsurf = (S, 16) if stage == "coarse" else (S - 16, 16)
+    masks = _voxel_masks(stage, "random") if compact else None
+    kw = dict(stage=stage, n_rays=n_rays, form=form, n_samples=ns, n_surface=nsurf, seed=3400 + n_rays, voxel_masks=masks)
+    with option(deterministic=det, wgrad_all=int(form == "all"), small_rays=0):
+        clean, names = render_call(**kw)
+        _poison_split_workspace(monkeypatch)
+        dirty, names_dirty = render_call(**kw)
+    check_kernels(names, stage, form, det)
+    check_kernels(names_dirty, stage, form, det)
+    what = "dirty %s N=%d S=%d %s compact=%d det=%d" % (stage, n_rays, S, form, compact, det)
+    if det:
+        assert_bits(dirty, clean, None, what)
+        return
+    assert_bits(dirty, clean, FWD, what)
+    for k in clean:
+        if k not in FWD:
+            assert bool(torch.isfinite(dirty[k]).all()), (what, k)
+            assert rel(dirty[k], clean[k]) < 1e-4, (what, k, rel(dirty[k], clean[k]))
+
+
+# ------------------------------------------------------------------------------------ the mode's dispatch edges
+def test_ray_group_family_backward_is_refused_by_name():
+    """S = 7 < kMinSamples takes the round-1 ray-group kernels, whose backward adds voxel gradients with atomics: the mode refuses it with an
+    error naming the option, before any backward kernel runs."""
+    from torch.profiler import ProfilerActivity, profile
+    sc, grids, dec_state = _scene()
+    with option(deterministic=1):
+        renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, n_samples=5, n_surface=2)
+        for p in dec.parameters():
+            p.requires_grad_(False)
+        ro, rd, gd, _ = (t.to(DEV) for t in su.make_rays(sc, 64, seed=3500))
+        c["grid_fine"] = c["grid_fine"].detach().clone().requires_grad_(True)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            depth, var, color = renderer.render_batch_ray(c, dec, rd, ro, DEV, "fine", gt_depth=gd)
+            with pytest.raises(RuntimeError, match="deterministic"):
+                depth.sum().backward()
+            torch.cuda.synchronize()
+    names = kernel_names(prof)
+    assert "render_fwd_tc_kernel" in names, names
+    assert not any(x.startswith("render_bwd") for x in names), names
+    assert c["grid_fine"].grad is None
+
+
+def test_small_rays_leaves_a_mapping_call_on_the_tile_kernels():
+    """small_rays = 64 would send a 16-ray call to the ray-group kernels; in deterministic mode a call with voxel and weight gradients stays on
+    the kDet tile backward, and its bits are those of small_rays = 0."""
+    runs = {}
+    for small in (64, 0):
+        with option(deterministic=1, small_rays=small):
+            runs[small], names = render_call("color", n_rays=16, form="color_wg", seed=3600)
+        check_kernels(names, "color", "color_wg", 1)
+    assert_bits(runs[64], runs[0], None, "small_rays")
+
+
+def test_tracking_call_runs_the_default_kernels():
+    """A tracking-form call (ray gradients only) has no order-dependent sum: deterministic mode leaves it on the default kernels, with the
+    bits of the mode off."""
+    sc, grids, dec_state = _scene()
+    runs = {}
+    for det in (1, 0):
+        with option(deterministic=det):
+            runs[det], names = _tracking_call(sc, grids, dec_state)
+        assert "render_bwd_tile_kernel" in names and not any("_det_" in x for x in names), (det, names)
+    assert_bits(runs[1], runs[0], ("depth", "var", "rgb", "d_rays_o", "d_rays_d"), "tracking")
+
+
+def _tracking_call(sc, grids, dec_state):
+    from test_gpu_wgrad_all import _profiled
+    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV)
+    for p in dec.parameters():
+        p.requires_grad_(False)                                   # (the fused tracker's form: the pose alone is optimised)
+    ro, rd, gd, gc = (t.to(DEV) for t in su.make_rays(sc, 200, seed=3700))
+    out = {}
+
+    def track():
+        r1 = ro.clone().requires_grad_(True)
+        r2 = rd.clone().requires_grad_(True)
+        depth, var, color = renderer.render_batch_ray(c, dec, r2, r1, DEV, "color", gt_depth=gd)
+        tp.tracking_loss(depth, var, color, gd, gc.double(), sc["tracking"]["w_color_loss"]).backward()
+        out.update(depth=depth.detach(), var=var.detach(), rgb=color.detach(), d_rays_o=r1.grad, d_rays_d=r2.grad)
+
+    names = _profiled(track)
+    return out, names
 
 
 # ------------------------------------------------------------------------------------ whole sequences

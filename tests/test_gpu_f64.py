@@ -29,10 +29,15 @@ METRICS = ("max", "l2", "pe_max", "pe_999")
 #    vs 4.5e-7), L2 18.8, per-element 25 (d_rays_o 1.7e-3 vs 6.8e-5).  3xTF32 drops lo*lo and the tensor core reads 10 mantissa bits of
 #    each part, so the kernel sits above float32 rounding while staying near 1e-5 in max norm;
 #  * fwd_f16 (colour stage; its backward is the 3xTF32 one): max 2.7 (soft grids x 30, var), L2 2.0, per-element 1.4.
+# Deterministic mode (option deterministic) is held to the same bars; its worst ratios over the det = 1 cases, (kernel - FLOOR) / port, on the
+# same H100: K max 8.9 (S = 127, var), L2 6.0, per-element 2.3 (S = 256, var); K_COARSE max 14.4, L2 18.6, per-element 25 (d_rays_o);
+# K_F16 max 2.7, L2 1.9, per-element 1.4 -- each equal to the default mode's, as the forward and the ray gradients are bit-identical.
 K = {"max": 14.0, "l2": 10.0, "pe_max": 6.0, "pe_999": 6.0}
 K_COARSE = {"max": 22.0, "l2": 28.0, "pe_max": 38.0, "pe_999": 38.0}
 K_F16 = {"max": 4.0, "l2": 3.0, "pe_max": 2.2, "pe_999": 2.2}
 #  * every decoder optimised (FP32-FMA backward), middle / fine / colour stages: max 6.8, L2 6.3, per-element 8.1 (init grids).
+#    Deterministic mode (kDet weight-gradient kernels, test_gpu_wgrad_all / test_gpu_mapper_settings): max 7.3 (colour stage N = 31,
+#    d_fine.fc_c.0.bias), L2 7.6 (fine + colour N = 64, d_fine.fc_c.4.bias), per-element 10.1 (fine stage x30, d_middle.fc_c.0.bias).
 K_FP32_PASS = {"max": 10.0, "l2": 10.0, "pe_max": 12.0, "pe_999": 12.0}
 FLOOR = {"max": 1e-7, "l2": 1e-7, "pe_max": 1e-6, "pe_999": 1e-6}
 BIAS_BAR = 8e-7     # measured fwd_f16 scale bias: occupancy -2.1e-7, colour -5.0e-7 (float32 port: 1.7e-8, 2.0e-9)
@@ -196,66 +201,99 @@ GRIDS = {"coarse": ("grid_coarse",), "middle": ("grid_middle",), "fine": ("grid_
 
 
 # ------------------------------------------------------------------------------------ tile residues, samples per ray, stages
-@pytest.mark.parametrize("n_rays", [128, 97, 95, 64, 33, 31, 1])
-def test_tile_residues_against_f64(n_rays):
+# Axes shared by the cases below: det = option deterministic (the kDet tile backward and the ordered sums of nsb_det.cu), held to the default
+# mode's bars -- both modes add the same float32 products, in another order; channels_last = False keeps the reference's NCDHW grids (the
+# strided gathers: gather_tile_strided, gather_tile_kt's strided branch, grid_load4's scalar loads in the scatter).
+LAYOUT = {True: "", False: " ncdhw"}
+
+
+def modes(cases, ncdhw=(), layout=True):
+    """pytest.param list over (case..., [channels_last,] det): every case in the default mode on channels-last grids under its own id, and in
+    deterministic mode ('-det'); the cases in `ncdhw` also on NCDHW grids ('-ncdhw', '-ncdhw-det')."""
+    def one(c, cl, det, suffix):
+        c = c if isinstance(c, tuple) else (c,)
+        return pytest.param(*(c + ((cl,) if layout else ()) + (det,)), id="-".join(str(v) for v in c) + suffix)
+    return [one(c, True, d, "-det" * d) for c in cases for d in (0, 1)] + \
+           [one(c, False, d, "-ncdhw" + "-det" * d) for c in ncdhw for d in (0, 1)]
+
+
+@pytest.mark.parametrize("n_rays,channels_last,det", modes([128, 97, 95, 64, 33, 31, 1], ncdhw=[97]))
+def test_tile_residues_against_f64(n_rays, channels_last, det):
     """S = 33 (17 + 16): N * S mod 128 = 0, 1, 63, 64, 65, 127 and one ray alone; rays and every stage grid through the tile backward."""
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, n_rays, seed=300 + n_rays)
-    check_case("residue N=%d" % n_rays, sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], n_samples=17, n_surface=16, seed=n_rays)
+    check_case("residue N=%d det=%d%s" % (n_rays, det, LAYOUT[channels_last]), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], n_samples=17,
+               n_surface=16, seed=n_rays, opts=dict(deterministic=det), channels_last=channels_last)
 
 
-@pytest.mark.parametrize("n_samples,n_surface,n_rays", [(8, 0, 40), (5, 4, 40), (111, 16, 20), (112, 16, 20), (113, 16, 20), (240, 16, 9)])
-def test_samples_per_ray_against_f64(n_samples, n_surface, n_rays):
+@pytest.mark.parametrize("n_samples,n_surface,n_rays,channels_last,det",
+                         modes([(8, 0, 40), (5, 4, 40), (111, 16, 20), (112, 16, 20), (113, 16, 20), (240, 16, 9)], ncdhw=[(240, 16, 9)]))
+def test_samples_per_ray_against_f64(n_samples, n_surface, n_rays, channels_last, det):
     """S from kMinSamples (8: 16 rays per tile) to NSB_MAX_SAMPLES (256: a ray over two tiles), 127 / 128 / 129 at the tile size."""
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, n_rays, seed=400 + n_samples)
-    check_case("S=%d" % (n_samples + n_surface), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], n_samples=n_samples, n_surface=n_surface,
-               seed=n_samples)
+    check_case("S=%d det=%d%s" % (n_samples + n_surface, det, LAYOUT[channels_last]), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"],
+               n_samples=n_samples, n_surface=n_surface, seed=n_samples, opts=dict(deterministic=det), channels_last=channels_last)
 
 
-@pytest.mark.parametrize("stage", ["coarse", "middle", "fine"])
-def test_stages_against_f64(stage):
-    """The occupancy stages through the tile kernels (coarse: MLP_no_xyz, no embedding -- the GEMMs alone set the error)."""
+@pytest.mark.parametrize("stage,channels_last,det", modes(["coarse", "middle", "fine"], ncdhw=["coarse"]))
+def test_stages_against_f64(stage, channels_last, det):
+    """The occupancy stages through the tile kernels (coarse: MLP_no_xyz, no embedding -- the GEMMs alone set the error; on NCDHW grids the
+    strided gather at the enlarged coarse bound)."""
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, 100, seed=500)
-    check_case("stage %s" % stage, sc, grids, dec, stage, ro, rd, gd, GRIDS[stage], seed=5)
+    check_case("stage %s det=%d%s" % (stage, det, LAYOUT[channels_last]), sc, grids, dec, stage, ro, rd, gd, GRIDS[stage], seed=5,
+               opts=dict(deterministic=det), channels_last=channels_last)
 
 
-@pytest.mark.parametrize("wgrad_tc", [1, 0])
-def test_colour_decoder_weight_gradients_against_f64(wgrad_tc):
-    """Mapping form of the colour stage: colour-decoder weight gradients on the tensor cores (render_bwd_wg_tile_kernel) and through
-    the FP32-FMA pass (wgrad_tc = 0); the ragged last tile at N * S = 97 * 48 (mod 128 = 48)."""
+@pytest.mark.parametrize("wgrad_tc,channels_last,det", [p for p in modes([1, 0], ncdhw=[1]) if p.id != "0-det"])
+def test_colour_decoder_weight_gradients_against_f64(wgrad_tc, channels_last, det):
+    """Mapping form of the colour stage: colour-decoder weight gradients on the tensor cores (render_bwd_wg_tile_kernel; deterministic mode:
+    render_bwd_wg_tile_det_kernel and the ordered tile sum; NCDHW grids: gather_tile_kt's strided branch) and through the FP32-FMA pass
+    (wgrad_tc = 0, which deterministic mode refuses); the ragged last tile at N * S = 97 * 48 (mod 128 = 48)."""
+    from nice_slam_b200 import _lib
+    if not wgrad_tc:
+        with options(wgrad_tc=0, deterministic=0):
+            assert _lib.lib().nsb_set_option(b"deterministic", 1) != 0
+            assert _lib.get_option("deterministic") == 0
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, 97, seed=600)
-    check_case("wgrad_tc=%d" % wgrad_tc, sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], ("color",), seed=6, opts=dict(wgrad_tc=wgrad_tc))
+    check_case("wgrad_tc=%d det=%d%s" % (wgrad_tc, det, LAYOUT[channels_last]), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], ("color",),
+               seed=6, opts=dict(wgrad_tc=wgrad_tc, deterministic=det), channels_last=channels_last)
 
 
-@pytest.mark.parametrize("split_model", [1, 0])
-def test_item_split_forms_against_f64(split_model):
+@pytest.mark.parametrize("split_model,det", modes([1, 0], layout=False))
+def test_item_split_forms_against_f64(split_model, det):
     """1408 rays x 48 = 528 tiles: with split_model = 1 tile_ws_plan takes one item per tile (all decoders in one CTA, full waves on 132
     SMs), with 0 one item per (tile, decoder)."""
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, 1408, seed=700)
-    check_case("split_model=%d" % split_model, sc, grids, dec, "color", ro, rd, gd, (), seed=7, opts=dict(split_model=split_model))
+    check_case("split_model=%d det=%d" % (split_model, det), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"] if det else (), seed=7,
+               opts=dict(split_model=split_model, deterministic=det))
 
 
 # ------------------------------------------------------------------------------------ value ranges
-@pytest.mark.parametrize("variant,scale", [("init", 1.0), ("soft", 1e-3), ("soft", 30.0)])
-def test_value_ranges_against_f64(variant, scale):
+@pytest.mark.parametrize("variant,scale,det", modes([("init", 1.0), ("soft", 1e-3), ("soft", 30.0)], layout=False))
+def test_value_ranges_against_f64(variant, scale, det):
     """Saturated scene (init grids: alpha = 1 at the first sample), tiny features (x 1e-3) and large ones (x 30)."""
     sc, grids, dec = scene(variant=variant, scale=scale)
     ro, rd, gd, _ = su.make_rays(sc, 100, seed=800)
-    check_case("%s x%g" % (variant, scale), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=8)
+    check_case("%s x%g det=%d" % (variant, scale, det), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=8, opts=dict(deterministic=det))
 
 
-def test_out_of_bound_and_zero_depth_rays_against_f64():
+def test_out_of_bound_and_zero_depth_rays_against_f64(det=0):
     """A batch mixing rays that start outside the bound (every sample occupancy 100), rays without a sensor depth and ordinary rays."""
     sc, grids, dec = scene()
     ro, rd, gd, _ = su.make_rays(sc, 90, seed=900)
     ro = ro.clone(); gd = gd.clone()
     ro[::3] += 100.0
     gd[1::4] = 0.0
-    check_case("oob + zero depth", sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=9)
+    check_case("oob + zero depth det=%d" % det, sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=9, opts=dict(deterministic=det))
+
+
+def test_out_of_bound_and_zero_depth_rays_in_deterministic_mode_against_f64():
+    """The same batch through the kDet tile backward and the ordered sums."""
+    test_out_of_bound_and_zero_depth_rays_against_f64(det=1)
 
 
 @pytest.mark.parametrize("stage,variant", [("middle", "soft"), ("fine", "soft"), ("color", "soft"), ("color", "init")])
@@ -275,14 +313,14 @@ def test_all_decoder_gradients_against_f64(stage, variant):
 
 
 # ------------------------------------------------------------------------------------ option fwd_f16
-@pytest.mark.parametrize("variant,scale", [("soft", 1.0), ("init", 1.0), ("soft", 30.0)])
-def test_fp16_split_forward_against_f64(variant, scale):
+@pytest.mark.parametrize("variant,scale,det", modes([("soft", 1.0), ("init", 1.0), ("soft", 30.0)], layout=False))
+def test_fp16_split_forward_against_f64(variant, scale, det):
     """Option fwd_f16 (FP16 hi | lo forward, DESIGN §4.4): 22 significant bits for operands in [2^-3, 65504], absolute 2^-25 below.  The
     init fine grid (sigma = 1e-4) is the absolute regime; soft x 30 drives activations into the tens."""
     sc, grids, dec = scene(variant=variant, scale=scale)
     ro, rd, gd, _ = su.make_rays(sc, 100, seed=1100)
-    check_case("f16 %s x%g" % (variant, scale), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=11, k_bar=K_F16, tau=1e-4,
-               opts=dict(fwd_f16=1))
+    check_case("f16 %s x%g det=%d" % (variant, scale, det), sc, grids, dec, "color", ro, rd, gd, GRIDS["color"], seed=11, k_bar=K_F16, tau=1e-4,
+               opts=dict(fwd_f16=1, deterministic=det))
 
 
 def test_fp16_split_forward_has_no_scale_bias():
@@ -312,11 +350,11 @@ def test_fp16_split_forward_has_no_scale_bias():
 
 
 # ------------------------------------------------------------------------------------ points mode
-def check_points(label, n_points, k_bar=K, k_bar_coarse=K_COARSE, opts=None):
+def check_points(label, n_points, k_bar=K, k_bar_coarse=K_COARSE, opts=None, channels_last=True):
     """FusedRenderer.eval_points at n_points points in and around the bound (seeded by n_points), coarse and colour stages, against
     fr.eval_points beside the float32 port."""
     sc, grids, dec_state = scene()
-    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV)
+    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, channels_last=channels_last)
     bound = su.scene_bound(sc)
     g = torch.Generator().manual_seed(n_points)
     lo, hi = bound[:, 0] - 0.2, bound[:, 1] + 0.2
@@ -340,10 +378,11 @@ def check_points(label, n_points, k_bar=K, k_bar_coarse=K_COARSE, opts=None):
     assert not failures, failures
 
 
-@pytest.mark.parametrize("n_points", [256, 129, 191, 192, 193, 255])
-def test_eval_points_against_f64(n_points):
-    """FusedRenderer.eval_points (points mode, one sample per 'ray'): point counts with residues 0, 1, 63, 64, 65, 127 mod 128."""
-    check_points("points", n_points)
+@pytest.mark.parametrize("n_points,channels_last,det", [p for p in modes([256, 129, 191, 192, 193, 255], ncdhw=[129]) if p.id == "129-ncdhw-det" or "det" not in p.id])
+def test_eval_points_against_f64(n_points, channels_last, det):
+    """FusedRenderer.eval_points (points mode, one sample per 'ray'): point counts with residues 0, 1, 63, 64, 65, 127 mod 128; NCDHW grids
+    through the strided gather, in both modes."""
+    check_points("points%s det=%d" % (LAYOUT[channels_last], det), n_points, opts=dict(deterministic=det), channels_last=channels_last)
 
 
 # ------------------------------------------------------------------------------------ option pdl

@@ -17,7 +17,7 @@ import scene_util as su
 from gpu_util import make_renderer, rel
 from oracle import f64_ref as fr
 from oracle import torch_port as tp
-from test_gpu_f64 import FLOOR, GRIDS, K_FP32_PASS, METRICS, check_masks, cotangents, kernel_run, scene, tensors
+from test_gpu_f64 import FLOOR, GRIDS, K_FP32_PASS, METRICS, check_masks, cotangents, kernel_run, modes, options, scene, tensors
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -30,6 +30,8 @@ TOL = 1e-4
 #    99.9th percentile 62 (output_linear.weight);
 #  * the same launch's rays, voxels and outputs at S = 33: max 24 (var), L2 27 (var), per-element 39 (d_rays_d) -- just above K_COARSE,
 #    which was measured at S = 32.
+# Deterministic mode (render_bwd_wg_coarse_tile_det_kernel, the per-tile partials summed in tile order), same H100, (kernel - FLOOR) / port:
+# max 32.7, L2 35.5, per-element 68.4, 99.9th percentile 59.8 -- the default mode's figures on the same cases.
 K_COARSE_WG = {"max": 50.0, "l2": 54.0, "pe_max": 104.0, "pe_999": 92.0}
 SOFT_FIXTURES = sorted(p for p in os.listdir(su.GOLDEN) if p.startswith("render_") and p.endswith(".pt") and "_soft" in p)
 
@@ -55,18 +57,19 @@ def kernel_names(prof):
 
 
 # ------------------------------------------------------------------------------------ float64 yardstick
-def check_all_decoders(label, stage, variant="soft", scale=1.0, n_rays=96, n_samples=None, n_surface=None, seed=0):
+def check_all_decoders(label, stage, variant="soft", scale=1.0, n_rays=96, n_samples=None, n_surface=None, seed=0, det=0, channels_last=True):
     """check_case of test_gpu_f64 with every decoder of the stage graded and option wgrad_all on: truth on the kernel's saved ReLU bits (the
     weight-gradient kernel reads them, as the input-gradient one does).  Bars: K_FP32_PASS, the bars every decoder's weight gradients are
-    held to; in the coarse stage K_COARSE_WG."""
+    held to; in the coarse stage K_COARSE_WG.  det = 1: option deterministic instead of wgrad_all (it implies it), whose kDet kernels and
+    ordered sums add the same products in another order, held to the same bars."""
     sc, grids, dec_state = scene(variant=variant, scale=scale)
     n_samples = sc["rendering"]["N_samples"] if n_samples is None else n_samples
     n_surface = sc["rendering"]["N_surface"] if n_surface is None else n_surface
     ro, rd, gd, _ = su.make_rays(sc, n_rays, seed=1600 + n_rays)
     decs = fr.STAGE_DECODERS[stage]
     cot = cotangents(n_rays, seed)
-    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, n_samples=n_samples, n_surface=n_surface)
-    with wgrad_all(1):
+    renderer, c, dec = make_renderer(sc, grids, dec_state, DEV, n_samples=n_samples, n_surface=n_surface, channels_last=channels_last)
+    with options(wgrad_all=1 - det, deterministic=det):
         kern = kernel_run(renderer, c, dec, ro, rd, gd, stage, cot, GRIDS[stage], decs)
     args = (grids, dec_state, ro, rd, stage, gd if stage != "coarse" else None, su.scene_bound(sc)) + cot
     kw = dict(grad_grids=GRIDS[stage], grad_decoders=decs, n_samples=n_samples, n_surface=n_surface)
@@ -90,27 +93,36 @@ def check_all_decoders(label, stage, variant="soft", scale=1.0, n_rays=96, n_sam
     assert not failures, "\n".join(failures)
 
 
-@pytest.mark.parametrize("stage", ["coarse", "middle", "fine", "color"])
-@pytest.mark.parametrize("n_rays", [97, 95, 64, 31])
-def test_all_decoder_weight_gradients_at_ragged_tiles_against_f64(n_rays, stage):
+@pytest.mark.parametrize("n_rays,stage,det", modes([(n, st) for n in (97, 95, 64, 31) for st in ("coarse", "middle", "fine", "color")], layout=False))
+def test_all_decoder_weight_gradients_at_ragged_tiles_against_f64(n_rays, stage, det):
     """S = 33 (17 + 16; the coarse stage, rendered without depth: 33 uniform samples): N * S mod 128 = 1, 63, 64, 127."""
     ns, nsurf = (33, 16) if stage == "coarse" else (17, 16)
-    check_all_decoders("wg all %s N=%d" % (stage, n_rays), stage, n_rays=n_rays, n_samples=ns, n_surface=nsurf, seed=n_rays)
+    check_all_decoders("wg all %s N=%d det=%d" % (stage, n_rays, det), stage, n_rays=n_rays, n_samples=ns, n_surface=nsurf, seed=n_rays, det=det)
 
 
+@pytest.mark.parametrize("det", [0, 1])
 @pytest.mark.parametrize("stage", ["coarse", "middle", "fine", "color"])
-def test_all_decoder_weight_gradients_on_large_features_against_f64(stage):
+def test_all_decoder_weight_gradients_on_ncdhw_grids_against_f64(stage, det):
+    """The reference's NCDHW grids (FusedRenderer(convert_grids=False)): the weight-gradient kernels gather the grid features through
+    gather_tile_kt's strided branch, the scatter through grid_load4's scalar loads; N * S = 97 * 33 (mod 128 = 1)."""
+    ns, nsurf = (33, 16) if stage == "coarse" else (17, 16)
+    check_all_decoders("wg all %s ncdhw det=%d" % (stage, det), stage, n_rays=97, n_samples=ns, n_surface=nsurf, seed=97, det=det,
+                       channels_last=False)
+
+
+@pytest.mark.parametrize("stage,det", modes(["coarse", "middle", "fine", "color"], layout=False))
+def test_all_decoder_weight_gradients_on_large_features_against_f64(stage, det):
     """Soft grids x 30 (activations in the tens)."""
-    check_all_decoders("wg all %s soft x30" % stage, stage, scale=30.0, seed=16)
+    check_all_decoders("wg all %s soft x30 det=%d" % (stage, det), stage, scale=30.0, seed=16, det=det)
 
 
-@pytest.mark.parametrize("stage", ["coarse", "middle"])
-def test_all_decoder_weight_gradients_in_the_saturated_scene_against_f64(stage):
+@pytest.mark.parametrize("stage,det", modes(["coarse", "middle"], layout=False))
+def test_all_decoder_weight_gradients_in_the_saturated_scene_against_f64(stage, det):
     """Init grids (alpha = 1 at the first sample).  Stages fine and colour are not claimed there: their decoders' weight gradients sit at the
     float32 noise floor, and one bias element each goes past K_FP32_PASS (measured on an H100: fine fc_c.0.bias 1.9e-3 in max norm against
     the port's 1.8e-4, 10.6x; colour fc_c.0.bias 2.4e-4 per element against 1.6e-5, 14x) -- the fine and colour decoders' kernel code is the
     one option wgrad_all does not change (test_gpu_mapper_settings does not claim this scene for the fine decoder either)."""
-    check_all_decoders("wg all %s init" % stage, stage, variant="init", seed=17)
+    check_all_decoders("wg all %s init det=%d" % (stage, det), stage, variant="init", seed=17, det=det)
 
 
 # ------------------------------------------------------------------------------------ reference fixtures
