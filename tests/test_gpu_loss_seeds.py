@@ -341,12 +341,13 @@ def test_tracking_seeds_at_every_entry_size(n):
 
 
 @gpu
-@pytest.mark.parametrize("n", [200, 777, 5000])
+@pytest.mark.parametrize("n", [200, 513, 777, 5000])
 def test_tracking_seeds_on_random_batches_with_a_pool_and_mapping_seeds(n):
-    """Random depth / variance / colour with missing sensor depths: own median, the median over an external pool of 1601 residuals (what a sharded
-    batch all-gathers), and the mapping seeds of the same batch."""
+    """Random depth / variance / colour with missing sensor depths: own median, no median gate (handle_dynamic 0), the median over an external
+    pool of 1601 residuals (what a sharded batch all-gathers), and the mapping seeds of the same batch."""
     b = random_batch(n)
     check_tracking(b)
+    check_tracking(b, handle_dynamic=0)
     pool = torch.rand(1601, generator=torch.Generator().manual_seed(10), dtype=F64) * 2.0
     want = check_tracking(b, pool=pool)
     assert want["loss"] > 0

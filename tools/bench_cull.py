@@ -15,7 +15,6 @@ import argparse
 import contextlib
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -29,46 +28,17 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
         sys.path.insert(0, p)
 
 from cull_scene import box_room, room_poses, write_ply_with_extras, write_traj   # noqa: E402
+from measure import Flush, card, log, median_spread, time_call                # noqa: E402
 
 STEPS = {"0.5M": 0.0109, "2M": 0.0054}                        # box_room grid steps: 0.50 M and 2.03 M vertices
 POSES = (200, 2000)
 
 
-def log(*a):
-    print(*a, file=sys.stderr, flush=True)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, check=True)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:                                    # (reported, not fatal)
-        return "unknown (%s)" % e
-
-
-def stats(vals):
-    return dict(median=float(np.median(vals)), spread=float(max(vals) - min(vals)))
-
-
 def kernel_round(v, f, w2c, flush):
     from nice_slam_b200.cull import cull_faces, cull_seen
-    t = {}
-
-    def timed(name, fn):
-        flush.zero_()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        out = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        t[name] = e0.elapsed_time(e1)
-        return out
-
-    seen = timed("seen_ms", lambda: cull_seen(v, w2c))
-    kept = timed("faces_ms", lambda: cull_faces(f, seen))
-    return t, seen, kept
+    seen, seen_ms, _ = time_call(lambda: cull_seen(v, w2c), flush)
+    kept, faces_ms, _ = time_call(lambda: cull_faces(f, seen), flush)
+    return dict(seen_ms=seen_ms, faces_ms=faces_ms), seen, kept
 
 
 def reference_loop(pc, poses):
@@ -100,7 +70,7 @@ def main():
     assert torch.cuda.is_available(), "bench_cull.py measures on the GPU"
     from nice_slam_b200 import cull
     res = dict(card=card(), rounds=a.rounds, ref_rounds=a.ref_rounds, cases=[])
-    flush = torch.empty(64 << 20, dtype=torch.float32, device="cuda")
+    flush = Flush()
     with tempfile.TemporaryDirectory() as tmp:
         for vname, step in STEPS.items():
             v, f = box_room(step)
@@ -134,8 +104,9 @@ def main():
                     torch.cuda.synchronize()
                     ref.append((time.perf_counter() - h0) * 1e3)
                 case = dict(vertices=int(len(v)), faces=int(len(f)), poses=P, unseen=float(1 - seen.mean()), kept_faces=int(len(kept)),
-                            seen_kernel_ms=stats([r[0]["seen_ms"] for r in rounds]), faces_kernel_ms=stats([r[0]["faces_ms"] for r in rounds]),
-                            cli_ms=stats(cli), reference_loop_ms=stats(ref) if ref else None,
+                            seen_kernel_ms=median_spread([r[0]["seen_ms"] for r in rounds]),
+                            faces_kernel_ms=median_spread([r[0]["faces_ms"] for r in rounds]),
+                            cli_ms=median_spread(cli), reference_loop_ms=median_spread(ref) if ref else None,
                             reference_mask_differs=int((ref_seen != seen.astype(bool)).sum()) if ref_seen is not None else None)
                 log("  " + json.dumps(case))
                 res["cases"].append(case)

@@ -15,7 +15,6 @@ python tools/bench_depth_l1.py [--rounds 5] [--host-rounds 2] [--views 1000] [--
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -27,22 +26,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-
-def log(*a):
-    print(*a, file=sys.stderr, flush=True)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, check=True)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:                                    # (reported, not fatal)
-        return "unknown (%s)" % e
-
-
-def stats(vals):
-    return dict(median=float(np.median(vals)), spread=float(max(vals) - min(vals)))
+from measure import card, log, median_spread, time_call                        # noqa: E402
 
 
 def furnished_room(step, n_boxes=24, seed=0):
@@ -87,19 +71,10 @@ def main():
             t0 = time.perf_counter()
             dp.sample_views(v, unseen, a.views, seed=0)
             t_views.append(time.perf_counter() - t0)
-        case["views"] = dict(stats([1e3 * t for t in t_views]), candidates=int(drawn), rejected=int(rejected), unseen_points=int(len(unseen)))
+        case["views"] = dict(median_spread([1e3 * t for t in t_views]), candidates=int(drawn), rejected=int(rejected), unseen_points=int(len(unseen)))
         dp.render_depth(v, f, c2w)                                     # warm-up
-        ms = []
-        for _ in range(a.rounds):
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            d = dp.render_depth(v, f, c2w)
-            e1.record()
-            torch.cuda.synchronize()
-            ms.append(e0.elapsed_time(e1))
-            del d
-        case["kernel_ms_per_mesh"] = stats(ms)
+        ms = [time_call(lambda: dp.render_depth(v, f, c2w))[1] for _ in range(a.rounds)]
+        case["kernel_ms_per_mesh"] = median_spread(ms)
         mv = transform_points(v, rigid(0.01, (0.0, 0.0, 1.0), (0.02, -0.01, 0.01)))
         eval_depth_l1((mv, f), (v, f), unseen, n_views=a.views)      # warm-up
         e2e, val = [], None
@@ -109,7 +84,7 @@ def main():
             val = eval_depth_l1((mv, f), (v, f), unseen, n_views=a.views)["depth_l1"]
             torch.cuda.synchronize()
             e2e.append(1e3 * (time.perf_counter() - t0))
-        case["e2e_ms"] = stats(e2e)
+        case["e2e_ms"] = median_spread(e2e)
         case["depth_l1_cm"] = val
         log("  " + json.dumps(case))
         res["sizes"].append(case)

@@ -16,6 +16,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 import scene_util as su                                       # noqa: E402
 from gpu_util import make_renderer                            # noqa: E402
+from measure import Flush, alternate, card, time_events       # noqa: E402
 from nice_slam_b200 import _lib                               # noqa: E402
 from nice_slam_b200.steps import IterationContext             # noqa: E402
 
@@ -39,34 +40,30 @@ def main():
     ap.add_argument("--rounds", type=int, default=20)
     ap.add_argument("--iters", type=int, default=20)
     a = ap.parse_args()
+    print("card: %s" % card(), flush=True)
     sc = su.load_scenes()["room0"]
     renderer, c, dec = make_renderer(sc, su.make_grids(sc, "soft"), su.load_decoders("soft"), DEV)
     for p in dec.parameters():
         p.requires_grad_(True)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=DEV)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    flush = Flush(DEV)
     props = torch.cuda.get_device_properties(0)
     out = {"gpu": props.name, "results": {}}
     for name, (kw, inputs) in workloads(sc, renderer).items():
         kw = dict(kw)
         n = kw.pop("n_rays")
         stage = kw.pop("stage")
-        ctxs, times = {}, {0: [], 1: []}
+        ctxs = {}
         for det in (0, 1):
             _lib.set_option("deterministic", det)
             ctxs[det] = IterationContext(renderer, n, stage, DEV, **kw)
             for _ in range(3):
                 ctxs[det].run(c, dec, *inputs)
-        for r in range(a.rounds):
-            for det in ((0, 1) if r % 2 == 0 else (1, 0)):
-                _lib.set_option("deterministic", det)
-                for _ in range(a.iters):
-                    flush.zero_()
-                    ev[0].record()
-                    ctxs[det].run(c, dec, *inputs)
-                    ev[1].record()
-                    ev[1].synchronize()
-                    times[det].append(ev[0].elapsed_time(ev[1]))
+
+        def run(det):
+            _lib.set_option("deterministic", det)
+            # one synchronize per call: the host enqueues each call on an idle device
+            return [time_events(lambda: ctxs[det].run(c, dec, *inputs), 1, flush=flush)[0] for _ in range(a.iters)]
+        times = {d: sum(r, []) for d, r in alternate((0, 1), a.rounds, run).items()}
         _lib.set_option("deterministic", 0)
         med = {d: sorted(t)[len(t) // 2] for d, t in times.items()}
         out["results"][name] = dict(default_ms=med[0], deterministic_ms=med[1], ratio=med[1] / med[0],

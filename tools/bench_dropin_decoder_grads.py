@@ -18,7 +18,6 @@ with the numbers.  Needs a CUDA device; there is no CPU fallback."""
 import argparse
 import collections
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,6 +28,7 @@ import torch  # noqa: E402
 import bench  # noqa: E402
 import scene_util as su  # noqa: E402
 from gpu_util import make_renderer  # noqa: E402
+from measure import Flush, alternate, card, stats, time_events  # noqa: E402
 from nice_slam_b200 import _lib  # noqa: E402
 from nice_slam_b200.mapping import tensor_from_c2w  # noqa: E402
 from oracle import torch_port as tp  # noqa: E402
@@ -36,15 +36,6 @@ from oracle import torch_port as tp  # noqa: E402
 STAGE_GRIDS = {"coarse": ("grid_coarse",), "middle": ("grid_middle",), "fine": ("grid_fine", "grid_middle"),
                "color": ("grid_fine", "grid_color", "grid_middle")}
 SETTINGS = (("frozen decoders", False, 0), ("trainable, wgrad_all=0", True, 0), ("trainable, wgrad_all=1", True, 1))
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[torch.cuda.current_device()]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return torch.cuda.get_device_name() + ", power limit and clocks unknown"
 
 
 def quad2rot(q):
@@ -63,19 +54,10 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_dropin_decoder_grads: needs a CUDA device")
+    print("card: %s" % card(), flush=True)
     dev = torch.device("cuda")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
     L = _lib.lib()
-
-    def time_steps(fn, warmup=5):
-        for _ in range(warmup):
-            fn()
-        torch.cuda.synchronize()
-        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.steps)]
-        for e0, e1 in evs:
-            flush.zero_(); e0.record(); fn(); e1.record()
-        torch.cuda.synchronize()
-        return sum(e0.elapsed_time(e1) for e0, e1 in evs) / a.steps
 
     def kernel_time(fn):
         """(render-kernel device ms per step, backward-launch device ms per step, backward kernel names) over a profiled run of its own"""
@@ -132,14 +114,15 @@ def main():
     cases = [("tracking iteration, 200 rays, stage color", track)]
     cases += [("mapping iteration, 996 rays, stage %s" % s, mapper(s)) for s in ("middle", "fine", "color")]
     cases += [("coarse mapper, 996 rays, stage coarse (no depth)", mapper("coarse"))]
-    rows = {}
-    for _ in range(a.rounds):
-        for label, trainable, wa in SETTINGS:
-            for p in dec.parameters():
-                p.requires_grad_(trainable)
-            _lib.check(L.nsb_set_option(b"wgrad_all", wa), "nsb_set_option")
-            for name, fn in cases:
-                rows.setdefault((name, label), []).append(time_steps(fn))
+
+    def run(setting):
+        label, trainable, wa = setting
+        for p in dec.parameters():
+            p.requires_grad_(trainable)
+        _lib.check(L.nsb_set_option(b"wgrad_all", wa), "nsb_set_option")
+        return [sum(time_events(fn, a.steps, warmup=5, flush=flush)) / a.steps for _, fn in cases]
+    per_setting = alternate(SETTINGS, a.rounds, run, reverse=False)
+    rows = {(name, s[0]): [r[i] for r in per_setting[s]] for s in SETTINGS for i, (name, _) in enumerate(cases)}
     kt = {}
     for label, trainable, wa in SETTINGS:
         for p in dec.parameters():
@@ -150,12 +133,11 @@ def main():
     _lib.check(L.nsb_set_option(b"wgrad_all", 0), "nsb_set_option")
     for p in dec.parameters():
         p.requires_grad_(True)
-    print("card: %s" % card())
     print("room0 soft, L2 flushed, CUDA events, %d steps x %d rounds: mean ms per step (min .. max over rounds) | device ms per step of the "
           "render kernels / of the backward launches (torch.profiler, %d steps, L2 not flushed) and the backward kernels" % (a.steps, a.rounds, a.profile_steps))
     for (name, label), v in rows.items():
         r, b, names = kt[(name, label)]
-        print("  %-52s %-24s %.4f  (%.4f .. %.4f) | %.4f / %.4f  %s" % (name, label, sum(v) / len(v), min(v), max(v), r, b, names))
+        print("  %-52s %-24s %.4f  (%.4f .. %.4f) | %.4f / %.4f  %s" % (name, label, *stats(v).values(), r, b, names))
 
 
 if __name__ == "__main__":

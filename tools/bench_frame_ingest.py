@@ -16,7 +16,6 @@ Reports the card, its power limit and the spread over rounds.  Needs a CUDA devi
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -30,6 +29,7 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 import yaml  # noqa: E402
 
+from measure import card  # noqa: E402
 from nice_slam_b200 import datasets as ds  # noqa: E402
 
 TUM_DIST = [0.2624, -0.9531, -0.0054, 0.0026, 1.1633]
@@ -41,11 +41,6 @@ FORMATS = {
     "scannet": dict(color=(968, 1296), depth=(480, 640), ext="jpg",
                     cam=dict(fx=577.59, fy=578.73, cx=318.91, cy=242.68, png_depth_scale=1000.0, crop_edge=10)),
 }
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip()
 
 
 def write_frames(folder, fmt, n):

@@ -13,7 +13,6 @@ Prints the card name and its power limit with the numbers.  Needs a CUDA device;
 import argparse
 import copy
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,19 +23,12 @@ import torch  # noqa: E402
 import bench  # noqa: E402
 import scene_util as su  # noqa: E402
 from gpu_util import make_renderer  # noqa: E402
+from measure import Flush, alternate, card, stats, time_events  # noqa: E402
 from nice_slam_b200 import _lib  # noqa: E402
 from nice_slam_b200.mapping import FusedMappingLoop  # noqa: E402
 from nice_slam_b200.steps import IterationContext  # noqa: E402
 
 GRIDS = {"fine": ("grid_fine", "grid_middle"), "color": ("grid_middle", "grid_fine", "grid_color")}
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[torch.cuda.current_device()]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return torch.cuda.get_device_name() + ", power limit unknown"
 
 
 def main():
@@ -46,18 +38,12 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_mapper_settings: needs a CUDA device")
+    print("card: %s" % card(), flush=True)
     dev = torch.device("cuda")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
 
-    def time_steps(fn, warmup=3):
-        for _ in range(warmup):
-            fn()
-        torch.cuda.synchronize()
-        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.steps)]
-        for e0, e1 in evs:
-            flush.zero_(); e0.record(); fn(); e1.record()
-        torch.cuda.synchronize()
-        return sum(e0.elapsed_time(e1) for e0, e1 in evs) / a.steps
+    def time_steps(fn):
+        return sum(time_events(fn, a.steps, warmup=3, flush=flush)) / a.steps
 
     sc = su.load_scenes()["room0"]
     renderer, c, dec = make_renderer(sc, su.make_grids(sc, "soft"), su.load_decoders("soft"), dev)
@@ -65,15 +51,15 @@ def main():
     ro, rd, dirs, gd, gc = [t.to(dev) for t in bench.make_batch(sc, n, 101)]
     gcf = gc.float()
     L = _lib.lib()
-    rows = {}
     iters = [("fine", ("fine",)), ("color", ("fine", "color")), ("color", ("color",))]
     ctxs = {(s, d): IterationContext(renderer, n, s, dev, kind="map", grad_grids=GRIDS[s], grad_decoders=d, host_staging=False) for s, d in iters}
-    for _ in range(a.rounds):
-        for tc in (1, 0):
-            _lib.check(L.nsb_set_option(b"wgrad_tc", tc), "nsb_set_option")
-            for (s, d), ctx in ctxs.items():
-                rows.setdefault("iteration stage %-5s grad_decoders=%-15s wgrad_tc=%d" % (s, "+".join(d), tc), []).append(
-                    time_steps(lambda: ctx.run(c, dec, ro, rd, gd, gcf)))
+
+    def run(tc):
+        _lib.check(L.nsb_set_option(b"wgrad_tc", tc), "nsb_set_option")
+        return [time_steps(lambda: ctx.run(c, dec, ro, rd, gd, gcf)) for ctx in ctxs.values()]
+    per_tc = alternate((1, 0), a.rounds, run, reverse=False)
+    rows = {"iteration stage %-5s grad_decoders=%-15s wgrad_tc=%d" % (s, "+".join(d), tc): [r[i] for r in per_tc[tc]]
+            for tc in (1, 0) for i, (s, d) in enumerate(ctxs)}
     _lib.check(L.nsb_set_option(b"wgrad_tc", 1), "nsb_set_option")
     depth1, color1 = su.make_frame(sc, 1)
     lr = dict(decoders=0.005, middle=0.005, fine=0.005, color=0.005)
@@ -92,10 +78,9 @@ def main():
     pc = color1[pj.long().cpu(), pi.long().cpu()].float().to(dev)
     rows["colour-refinement loop step (BA, 6 x 166 rays)"] = [time_steps(lambda: loop.iteration_ba("color", pi, pj, pd, pc, lr))
                                                                for _ in range(a.rounds)]
-    print("card: %s" % card())
     print("996 rays, room0 soft, L2 flushed, CUDA events, %d steps x %d rounds: mean ms per step (min .. max over rounds)" % (a.steps, a.rounds))
     for label, v in rows.items():
-        print("  %-62s %.4f  (%.4f .. %.4f)" % (label, sum(v) / len(v), min(v), max(v)))
+        print("  %-62s %.4f  (%.4f .. %.4f)" % (label, *stats(v).values()))
 
 
 if __name__ == "__main__":

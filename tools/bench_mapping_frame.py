@@ -18,18 +18,17 @@ import argparse
 import json
 import os
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import scene_util as su  # noqa: E402
-from bench_dropin_decoder_grads import card, quad2rot  # noqa: E402
+from bench_dropin_decoder_grads import quad2rot  # noqa: E402
 from gpu_util import make_renderer  # noqa: E402
+from measure import Flush, alternate, card, stats, time_call  # noqa: E402
 from nice_slam_b200 import FusedMapper  # noqa: E402
 from nice_slam_b200.keyframes import KeyframeStore  # noqa: E402
 from nice_slam_b200.mapping import map_stage, stage_lrs, tensor_from_c2w, window_rows  # noqa: E402
@@ -121,7 +120,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_mapping_frame: needs a CUDA device")
     dev = torch.device("cuda")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
     sc = su.load_scenes()["room0"]
     cam = sc["cam"]
     renderer, c, dec = make_renderer(sc, su.make_grids(sc, "soft"), su.load_decoders("soft"), dev)
@@ -150,22 +149,12 @@ def main():
         for fn in arms.values():                                        # warm-up: module loads, allocator, autograd
             fn(); fn()
         torch.cuda.synchronize()
-        times = {k: dict(event=[], wall=[]) for k in arms}
-        for _ in range(a.rounds):
-            for arm, fn in arms.items():
-                for _ in range(a.calls):
-                    flush.zero_()
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    e0.record(); fn(); e1.record()
-                    torch.cuda.synchronize()
-                    times[arm]["wall"].append((time.perf_counter() - t0) * 1e3)
-                    times[arm]["event"].append(e0.elapsed_time(e1))
+        per_round = alternate(tuple(arms), a.rounds, lambda arm: [time_call(arms[arm], flush)[1:] for _ in range(a.calls)], reverse=False)
+        times = {k: dict(event=[e for r in v for e, _ in r], wall=[w for r in v for _, w in r]) for k, v in per_round.items()}
         row = dict(workload=name, iters=a.iters, pixels=s["pixels"], window_rows=len(selection) + 2, calls_per_arm=a.rounds * a.calls)
         for arm, t in times.items():
             for kind, v in t.items():
-                row["%s_%s_ms" % (arm, kind)] = dict(mean=round(sum(v) / len(v), 3), min=round(min(v), 3), max=round(max(v), 3))
+                row["%s_%s_ms" % (arm, kind)] = {k: round(x, 3) for k, x in stats(v).items()}
         row["speedup_wall"] = round(row["drop-in_wall_ms"]["mean"] / row["fused_wall_ms"]["mean"], 2)
         results.append(row)
         print(json.dumps(row))

@@ -9,7 +9,6 @@ python tools/bench_mesh.py [--rounds 5] [--keyframes 10] [--out results/bench_me
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -24,32 +23,18 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 import scene_util as su                                       # noqa: E402
 from gpu_util import make_renderer                            # noqa: E402
+from measure import Flush, card, median_spread, time_call     # noqa: E402
 
 PHASES = ("hull", "lattice", "marching_cubes", "masks", "components", "colors", "ply_write")
 MC_BOUND = [[-2.9, 8.9], [-3.2, 5.5], [-3.5, 3.3]]          # configs/Replica/room0.yaml
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:                                    # (reported, not fatal)
-        return "unknown (%s)" % e
 
 
 def one_round(mesher, c, dec, store, est, flush, tmpdir):
     t = {}
 
     def timed(name, fn):
-        flush.zero_()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        h0 = time.perf_counter()
-        e0.record()
-        out = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        t[name] = dict(events_ms=e0.elapsed_time(e1), host_ms=(time.perf_counter() - h0) * 1e3)
+        out, events_ms, host_ms = time_call(fn, flush)
+        t[name] = dict(events_ms=events_ms, host_ms=host_ms)
         return out
 
     with torch.no_grad():
@@ -86,7 +71,7 @@ def main():
         depth, color = su.make_frame(sc, 500 + k)
         store.append(k, color, depth, su.make_pose(sc, 500 + k))
     est = torch.stack(store.est_c2w)
-    flush = torch.empty(64 << 20, dtype=torch.float32, device="cuda")
+    flush = Flush()
     res = dict(card=card(), keyframes=a.keyframes, rounds=a.rounds, resolutions={})
     with tempfile.TemporaryDirectory() as tmpdir:
         for R in a.resolutions:
@@ -101,10 +86,9 @@ def main():
                 for kind in ("events_ms", "host_ms"):
                     vals = [r[0][ph][kind] for r in rounds if r[0][ph][kind] is not None]
                     if vals:
-                        summary.setdefault(ph, {})[kind] = dict(median=float(np.median(vals)), spread=float(max(vals) - min(vals)))
+                        summary.setdefault(ph, {})[kind] = median_spread(vals)
             total = [sum(r[0][ph]["host_ms"] for ph in PHASES) for r in rounds]
-            res["resolutions"][R] = dict(phases=summary, total_host_ms=dict(median=float(np.median(total)), spread=float(max(total) - min(total))),
-                                         sizes=rounds[0][1])
+            res["resolutions"][R] = dict(phases=summary, total_host_ms=median_spread(total), sizes=rounds[0][1])
     line = json.dumps(res)
     print(line)
     if a.out:

@@ -14,8 +14,6 @@ in the order given.  Prints the card name and its power limit with the numbers. 
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,19 +22,12 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 
 import bench  # noqa: E402
+from measure import Flush, alternate, card, stats, time_events  # noqa: E402
 from nice_slam_b200 import _lib  # noqa: E402
 from nice_slam_b200.steps import IterationContext  # noqa: E402
 
 TRACK_RAYS = (16, 64, 200, 1000)
 MAP_RAYS = 996
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[torch.cuda.current_device()]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return torch.cuda.get_device_name() + ", power limit unknown"
 
 
 def set_backend(b):
@@ -51,8 +42,9 @@ def main():
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda", 0)
+    gpu = card()
     sc, renderer, c, dec = bench.build_scene(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
 
     # (workload, backend) -> graph; the contexts stay alive as long as their graphs
     graphs, keep = {}, []
@@ -74,30 +66,17 @@ def main():
             keep.append(ctx)
     set_backend(0)
 
-    def time_graph(g):
-        for _ in range(20):
-            g.replay()
-        torch.cuda.synchronize()
-        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
-        for a, e in evs:
-            flush.zero_(); a.record(); g.replay(); e.record()
-        torch.cuda.synchronize()
-        return sum(a.elapsed_time(e) for a, e in evs) / args.steps
-
-    ms = {k: [] for k in graphs}
-    for _ in range(args.rounds):
-        for name, _n in work:
-            for b in args.backends:
-                ms[name, b].append(time_graph(graphs[name, b]))
+    ms = alternate(tuple(graphs), args.rounds, lambda k: sum(time_events(graphs[k].replay, args.steps, warmup=20, flush=flush)) / args.steps,
+                   reverse=False)
     rows = []
     for name, _n in work:
         row = {"workload": name}
         for b in args.backends:
             v = ms[name, b]
-            row["mlp_backend_%d" % b] = {"mean_ms": statistics.mean(v), "min_ms": min(v), "max_ms": max(v), "rounds": [round(x, 4) for x in v]}
+            row["mlp_backend_%d" % b] = {**{k + "_ms": x for k, x in stats(v).items()}, "rounds": [round(x, 4) for x in v]}
         rows.append(row)
-    print(json.dumps({"card": card(), "steps": args.steps, "rounds": args.rounds, "results": rows}, indent=1))
-    print("card: %s" % card())
+    print(json.dumps({"card": gpu, "steps": args.steps, "rounds": args.rounds, "results": rows}, indent=1))
+    print("card: %s" % gpu)
     print("%-10s" % "workload" + "".join("  backend %d: mean [min, max] ms" % b for b in args.backends))
     for row in rows:
         print("%-10s" % row["workload"] + "".join("  %8.4f [%.4f, %.4f]" % (row["mlp_backend_%d" % b]["mean_ms"], row["mlp_backend_%d" % b]["min_ms"],

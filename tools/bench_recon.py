@@ -12,7 +12,6 @@ python tools/bench_recon.py [--rounds 5] [--host-rounds 1] [--out results/bench_
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,22 +25,11 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 import scene_util as su                                       # noqa: E402
 from gpu_util import make_renderer                            # noqa: E402
+from measure import Flush, card, log, median_spread, time_call  # noqa: E402
 from oracle import recon as orc                               # noqa: E402
 
 MC_BOUND = [[-2.9, 8.9], [-3.2, 5.5], [-3.5, 3.3]]          # configs/Replica/room0.yaml
 N_SAMPLES = 200000
-
-
-def log(*a):
-    print(*a, file=sys.stderr, flush=True)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:                                    # (reported, not fatal)
-        return "unknown (%s)" % e
 
 
 def meshes(resolutions, keyframes=10):
@@ -78,15 +66,8 @@ def gpu_round(rv, rf, gv, gf, flush):
     t = {}
 
     def timed(name, fn):
-        flush.zero_()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        h0 = time.perf_counter()
-        e0.record()
-        out = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        t[name] = dict(events_ms=e0.elapsed_time(e1), host_ms=(time.perf_counter() - h0) * 1e3)
+        out, events_ms, host_ms = time_call(fn, flush)
+        t[name] = dict(events_ms=events_ms, host_ms=host_ms)
         return out
 
     dev = torch.device("cuda")
@@ -135,7 +116,7 @@ def summarise(rounds):
     for ph in rounds[0]:
         for k, v0 in rounds[0][ph].items():
             vals = [r[ph][k] for r in rounds]
-            out.setdefault(ph, {})[k] = v0 if k == "iterations" else dict(median=float(np.median(vals)), spread=float(max(vals) - min(vals)))
+            out.setdefault(ph, {})[k] = v0 if k == "iterations" else median_spread(vals)
     return out
 
 
@@ -148,7 +129,7 @@ def main():
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_recon.py measures on the GPU"
     res = dict(card=card(), n_samples=N_SAMPLES, rounds=a.rounds, host_rounds=a.host_rounds, resolutions={})
-    flush = torch.empty(64 << 20, dtype=torch.float32, device="cuda")
+    flush = Flush()
     for R, (gv, gf) in meshes(a.resolutions).items():
         rv = moved(gv)
         log("resolution %d: %d vertices, %d faces" % (R, len(gv), len(gf)))

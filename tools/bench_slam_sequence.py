@@ -12,7 +12,6 @@ Needs a CUDA device; there is no CPU fallback."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -23,6 +22,7 @@ import torch  # noqa: E402
 
 import scene_util as su  # noqa: E402
 from gpu_util import make_renderer  # noqa: E402
+from measure import card  # noqa: E402
 from nice_slam_b200 import FusedSLAM, ate_rmse  # noqa: E402
 from slam_sequences import path_pose  # noqa: E402
 
@@ -37,11 +37,6 @@ MAPPING = dict(pixels=1000, mapping_window_size=5, middle_iter_ratio=0.4, fine_i
                keyframe_every=50, ckpt_freq=500, no_log_on_first_frame=True, iters=60, iters_first=1500, lr_factor=1.0, lr_first_factor=5.0,
                color_refine=True, BA=True, save_selected_keyframes_info=False)
 CFG = dict(tracking=TRACKING, mapping=MAPPING, coarse=True, sync_method="strict")
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip()
 
 
 def frames_for(sc, n):
@@ -72,6 +67,7 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_slam_sequence: needs a CUDA device")
+    gpu = card()
     sc = su.load_scenes()["room0"]
     frames = frames_for(sc, a.frames)
     warm = dict(CFG, mapping=dict(MAPPING, iters_first=20, iters=10))
@@ -90,7 +86,7 @@ def main():
     b_total, _, b_ate = one_run(sc, frames, cfg=base)
     print("baseline (1 mapping iteration per call): %.3f s  ATE %.4f m" % (b_total, b_ate), flush=True)
     tot = [x["total_s"] for x in rounds]
-    res = dict(card=card(), frames=a.frames, rounds=rounds, total_s_min=min(tot), total_s_max=max(tot),
+    res = dict(card=gpu, frames=a.frames, rounds=rounds, total_s_min=min(tot), total_s_max=max(tot),
                spread=(max(tot) - min(tot)) / min(tot), fps=a.frames / min(tot), ate_m=rounds[0]["ate_m"],
                baseline_one_mapping_iteration=dict(total_s=b_total, ate_m=b_ate))
     print(json.dumps(res))

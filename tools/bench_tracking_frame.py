@@ -16,17 +16,16 @@ import argparse
 import json
 import os
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 import scene_util as su  # noqa: E402
-from bench_dropin_decoder_grads import card, quad2rot  # noqa: E402
+from bench_dropin_decoder_grads import quad2rot  # noqa: E402
 from gpu_util import make_renderer  # noqa: E402
+from measure import Flush, alternate, card, stats, time_call  # noqa: E402
 from nice_slam_b200.mapping import tensor_from_c2w  # noqa: E402
 from nice_slam_b200.tracking import FusedTrackingLoop  # noqa: E402
 from oracle import torch_port as tp  # noqa: E402
@@ -79,7 +78,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_tracking_frame: needs a CUDA device")
     dev = torch.device("cuda")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
     sc = su.load_scenes()["room0"]
     renderer, c, dec = make_renderer(sc, su.make_grids(sc, "soft"), su.load_decoders("soft"), dev)
     for p in dec.parameters():
@@ -98,22 +97,12 @@ def main():
         for fn in arms.values():                                        # warm-up: module loads, allocator, autograd
             fn(); fn()
         torch.cuda.synchronize()
-        times = {k: dict(event=[], wall=[]) for k in arms}
-        for _ in range(a.rounds):
-            for name, fn in arms.items():
-                for _ in range(n_frames):
-                    flush.zero_()
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    e0.record(); fn(); e1.record()
-                    torch.cuda.synchronize()
-                    times[name]["wall"].append((time.perf_counter() - t0) * 1e3)
-                    times[name]["event"].append(e0.elapsed_time(e1))
+        per_round = alternate(tuple(arms), a.rounds, lambda arm: [time_call(arms[arm], flush)[1:] for _ in range(n_frames)], reverse=False)
+        times = {k: dict(event=[e for r in v for e, _ in r], wall=[w for r in v for _, w in r]) for k, v in per_round.items()}
         row = dict(iters=iters, pixels=pixels, frames_per_arm=a.rounds * n_frames)
         for name, t in times.items():
             for kind, v in t.items():
-                row["%s_%s_ms" % (name, kind)] = dict(mean=round(sum(v) / len(v), 3), min=round(min(v), 3), max=round(max(v), 3))
+                row["%s_%s_ms" % (name, kind)] = {k: round(x, 3) for k, x in stats(v).items()}
         row["speedup_wall"] = round(row["drop-in_wall_ms"]["mean"] / row["loop_wall_ms"]["mean"], 2)
         results.append(row)
         print(json.dumps(row))

@@ -91,9 +91,13 @@ def compare(a_path, b_path):
     return 1 if bad else 0
 
 
-if __name__ == "__main__":
+def main():
     if len(sys.argv) == 4 and sys.argv[1] == "--compare":
         sys.exit(compare(sys.argv[2], sys.argv[3]))
     if len(sys.argv) != 2:
         sys.exit(__doc__)
     dump(sys.argv[1])
+
+
+if __name__ == "__main__":
+    main()

@@ -22,9 +22,10 @@ from collections import Counter, defaultdict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-os.environ.setdefault("NSB_LIB", os.path.join(ROOT, "nice_slam_b200", "libnsb_items.so"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+
+from measure import Flush  # noqa: E402
 
 LAUNCHES = ("forward", "backward", "weight-gradient backward")
 LEVEL_NAMES = {-1: "all", 0: "coarse", 1: "middle", 2: "fine", 3: "color"}
@@ -41,7 +42,8 @@ def read_records(fn, launch):
     return buf[:n].copy()
 
 
-def stats(v):
+def latency_stats(v):
+    """count, mean, median, min and max of a list of microsecond figures, which may be empty"""
     return {"n": len(v), "mean_us": statistics.mean(v), "median_us": statistics.median(v), "min_us": min(v), "max_us": max(v)} if v else {"n": 0}
 
 
@@ -84,13 +86,13 @@ def analyse(runs, sms):
             return "+".join(sorted(kinds[x] for x in by_sm[int(rec["sm"][b])]))
         last_exit[on_sm(int(np.argmax(t2)))] += 1
         last_chain[on_sm(int(np.argmax(t1)))] += 1
-    return {"blocks": len(runs[0]), "iterations": len(runs), "launch_span_us": stats(spans),
-            "item_latency_us": {k: {s: stats(v[s]) for s in v} for k, v in sorted(lat.items())},
-            "chain_latency_us": {k: {s: stats(v[s]) for s in v} for k, v in sorted(chain.items())},
+    return {"blocks": len(runs[0]), "iterations": len(runs), "launch_span_us": latency_stats(spans),
+            "item_latency_us": {k: {s: latency_stats(v[s]) for s in v} for k, v in sorted(lat.items())},
+            "chain_latency_us": {k: {s: latency_stats(v[s]) for s in v} for k, v in sorted(chain.items())},
             "sharing_pairs_per_launch": {k: v / len(runs) for k, v in pairs.most_common()},
             "dispatch": {"first_round_one_block_per_sm": sum(first_round_distinct) / len(runs),
                          "block_m_plus_j_on_sm_of_block_j": (second_round_same / second_round_n) if second_round_n else None,
-                         "first_round_start_spread_us": stats(start_spread),
+                         "first_round_start_spread_us": latency_stats(start_spread),
                          "first_round_sm_order_of_one_launch": [int(s) for s in runs[-1]["sm"][:min(len(runs[-1]), sms)]]},
             "last_sm_by_exit": dict(last_exit.most_common()), "last_sm_by_chain_end": dict(last_chain.most_common())}
 
@@ -119,6 +121,7 @@ def main():
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--out", default="item_timing")
     args = ap.parse_args()
+    os.environ.setdefault("NSB_LIB", os.path.join(ROOT, "nice_slam_b200", "libnsb_items.so"))       # before nice_slam_b200._lib loads
     import bench
     from nice_slam_b200 import _lib
     from nice_slam_b200.steps import IterationContext
@@ -129,7 +132,7 @@ def main():
     fn.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int]
     props = torch.cuda.get_device_properties(dev)
     sms = props.multi_processor_count
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    flush = Flush(dev)
     os.makedirs(args.out, exist_ok=True)
     result = {"device": props.name, "sms": sms, "workloads": {}}
     lines = ["%s, %d SMs; %d iterations per workload, L2 flushed before each" % (props.name, sms, args.iters)]
@@ -147,7 +150,7 @@ def main():
         runs = defaultdict(list)
         for _ in range(args.iters):
             fn(0, None, 0, 1)
-            flush.zero_()
+            flush.flush()
             step()
             torch.cuda.synchronize()
             for launch in range(3):

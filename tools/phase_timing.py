@@ -7,12 +7,6 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-os.environ.setdefault("NSB_LIB", os.path.join(ROOT, "nice_slam_b200", "libnsb_timing.so"))
-import torch  # noqa: E402
-import scene_util as su  # noqa: E402
-from gpu_util import make_renderer  # noqa: E402
-from nice_slam_b200 import _lib  # noqa: E402
-from nice_slam_b200.steps import IterationContext  # noqa: E402
 
 TILE_NAMES = {40: "fwd: launch -> depth max done", 41: "fwd: ray table (bbox far, near)", 43: "fwd: sample z + rank sort", 44: "fwd: point geometry + syncs",
               1: "fwd: gather (per grid)", 5: "fwd: publish + wait all warps' gather", 11: "fwd: wait fc_c weight units (TMA)",
@@ -32,6 +26,12 @@ NAMES = {0: "fwd: tail sync of previous decoder", 1: "fwd: gather", 2: "fwd: fc_
 
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 200
+    os.environ.setdefault("NSB_LIB", os.path.join(ROOT, "nice_slam_b200", "libnsb_timing.so"))       # before nice_slam_b200._lib loads
+    import torch
+    import scene_util as su
+    from gpu_util import make_renderer
+    from nice_slam_b200 import _lib
+    from nice_slam_b200.steps import IterationContext
     dev = torch.device("cuda")
     sc = su.load_scenes()["room0"]
     renderer, c, dec = make_renderer(sc, su.make_grids(sc, "soft"), su.load_decoders("soft"), dev)

@@ -8,7 +8,6 @@ the colour / fine / middle grids and the colour decoder, as in a colour mapping 
 import argparse
 import json
 import os
-import subprocess
 import sys
 from types import SimpleNamespace
 
@@ -19,18 +18,11 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import scene_util as su                                   # noqa: E402
 from gpu_util import make_cfg                             # noqa: E402
+from measure import card, time_events                     # noqa: E402
 from nice_slam_b200.decoders import NICEDecoders           # noqa: E402
 from nice_slam_b200.renderer import FusedRenderer          # noqa: E402
 
 CASES = {"default": {}, "perturb": dict(perturb=1.0), "lindisp": dict(lindisp=True), "importance12": dict(N_importance=12)}
-
-
-def card():
-    try:
-        q = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], text=True)
-        return q.strip().splitlines()[0]
-    except (OSError, subprocess.CalledProcessError):
-        return torch.cuda.get_device_name(0) + ", power limit unknown"
 
 
 def main():
@@ -68,14 +60,8 @@ def main():
                 (depth.sum() + var.sum() + rgb.sum()).backward()
             for _ in range(a.warmup):
                 step()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(a.iters):
-                step()
-            e1.record()
-            torch.cuda.synchronize()
-            ms = e0.elapsed_time(e1) / a.iters
+            # one event pair around all the calls: the gaps between calls (host-side autograd) count
+            ms = time_events(lambda: [step() for _ in range(a.iters)], 1)[0] / a.iters
             print(json.dumps(dict(rays=n, sampling=name, ms_fwd_bwd=round(ms, 4), iters=a.iters)))
 
 
